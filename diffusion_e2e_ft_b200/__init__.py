@@ -1,9 +1,9 @@
-"""diffusion_e2e_ft_b200 — B200-native single-step denoising engine (UNet2DConditionModel + AutoencoderKL
+"""diffusion_e2e_ft_b200 — H100-native single-step denoising engine (UNet2DConditionModel + AutoencoderKL
 hot path of VisualComputingInstitute/diffusion-e2e-ft) behind the reference's module / pipeline API.
 
     from diffusion_e2e_ft_b200 import B200UNet2DConditionModel, B200AutoencoderKL, MarigoldPipeline
 
-Arithmetic lives in libb200_e2eft.so (hand-written sm_100a CUDA, C ABI in include/b200_e2eft.h).
+Arithmetic lives in libb200_e2eft.so (hand-written sm_90a CUDA, C ABI in include/b200_e2eft.h).
 """
 from .lib import load as load_library, LIB_PATH, EXPORTS  # noqa: F401
 from .unet import B200UNet2DConditionModel, UNet2DConditionOutput  # noqa: F401

@@ -2,7 +2,7 @@
 
 The reference trains through `accelerator.backward(loss)` (training/train.py:563): plain torch.autograd over
 the UNet and the frozen VAE decoder.  The engine keeps that boundary: every block of modules.py / unet.py is one
-`torch.autograd.Function` whose forward runs the same sm_100a kernels as inference (saving the operands the
+`torch.autograd.Function` whose forward runs the same sm_90a kernels as inference (saving the operands the
 backward needs) and whose backward is hand-written on the backward operators of backward.py / csrc/backward.cu.
 torch.autograd is used for what it is in the reference — graph bookkeeping between blocks (skip connections,
 the shared time embedding, `.grad` accumulation) — never for arithmetic inside a block.

@@ -1,13 +1,13 @@
 """Backward-pass operators of the fine-tuning step (SURVEY.md §8 row a10; reference training/train.py:545-566,
-`accelerator.backward(loss)`), composed from the tcgen05 GEMM / implicit-GEMM conv kernels with transposed or
+`accelerator.backward(loss)`), composed from the wgmma GEMM / implicit-GEMM conv kernels with transposed or
 re-packed operands plus the streaming kernels in csrc/backward.cu.  Every function here is checked against
-torch.autograd on the B200 (tests/kernel_checks.py, `bwd_*`).
+torch.autograd on the GPU (tests/kernel_checks.py, `bwd_*`).
 
 Conventions: activations / incoming gradients that feed a GEMM are fp16 (the training step multiplies the loss
 by a static loss scale so they stay in range), parameter gradients are fp32, the gradient of the residual stream
 is fp32 unless stated.  Weight-gradient GEMMs contract over pixels (K = NB*H*W): both operands are brought into
 K-major form by `ops.gather_planar` (one pass each; a later version reads them MN-major straight from the
-NHWC tensors through the UMMA descriptor, like V in the attention kernel).
+NHWC tensors through the wgmma descriptor, like V in the attention kernel).
 """
 import torch
 
@@ -30,7 +30,7 @@ def linear_bwd(a, w, dy, need_da=True, da_dtype=F16, da_add=None, need_dw=True, 
     if need_dw:
         # dw = dy^T @ a: both operands are stored [contraction = M rows][columns] -> MN-major A and B, no transposes.
         # An [N x K] output is only a handful of 128 x 256 tiles: split the row contraction over `S` batches (views of
-        # the same buffers) so the GEMM fills the 148 SMs, then fold the partial sums.
+        # the same buffers) so the GEMM fills the 132 SMs, then fold the partial sums.
         S = _row_splits(M, N, K)
         if S > 1 and dy.stride(1) == 1 and a.stride(1) == 1:
             mc = M // S
@@ -45,7 +45,7 @@ def linear_bwd(a, w, dy, need_da=True, da_dtype=F16, da_add=None, need_dw=True, 
     return da, dw, db
 
 
-def _row_splits(M, N, K, target_ctas=296, min_rows=512):
+def _row_splits(M, N, K, target_ctas=264, min_rows=512):
     """Number of equal row chunks (a divisor of M / 64) for a split-K weight-gradient GEMM of an [N x K] output."""
     if M % 64 != 0:
         return 1
@@ -60,15 +60,16 @@ def _row_splits(M, N, K, target_ctas=296, min_rows=512):
 
 
 # -------------------------------------------------------------------------------------------------- conv
-# Weight-gradient GEMM variants (GPU-verified in round 2: tests/test_engine_gpu.py::test_wgrad_variants; defaults chosen
-# from tools/train_step_timing.py on a B200, overridable with B200_WGRAD_PADDED / B200_WGRAD_SPLIT_K):
+# Weight-gradient GEMM variants (GPU-verified: tests/test_engine_gpu.py::test_wgrad_variants; overridable with
+# B200_WGRAD_PADDED / B200_WGRAD_SPLIT_K):
 #   WGRAD_PADDED  stride-1 3x3 convs: one zero-padded planar copy of X and three column-shifted copies of dY instead
 #                 of nine shifted copies of X; a kernel row (ky) is a 16-byte-aligned pointer offset of ky*Wp into X.
-#   WGRAD_SPLIT_K split the pixel contraction over `batch` so a Cout x Cin weight-gradient GEMM fills the 148 SMs;
-#                 value = target number of CTAs (0 = no split); partial sums are reduced by `col_sum`.
+#   WGRAD_SPLIT_K split the pixel contraction over `batch` so a Cout x Cin weight-gradient GEMM fills the 132 SMs;
+#                 value = target number of CTAs (0 = no split, default two waves of 132); partial sums are reduced by
+#                 `col_sum`.
 import os as _os
-WGRAD_PADDED = _os.environ.get("B200_WGRAD_PADDED", "1") == "1"       # r2, bs 2 768^2: 262 -> 254 ms / iteration with both on
-WGRAD_SPLIT_K = int(_os.environ.get("B200_WGRAD_SPLIT_K", "296"))
+WGRAD_PADDED = _os.environ.get("B200_WGRAD_PADDED", "1") == "1"
+WGRAD_SPLIT_K = int(_os.environ.get("B200_WGRAD_SPLIT_K", "264"))
 WGRAD_MIN_KBLOCKS = 8        # at least this many 64-wide k-blocks per split
 
 
@@ -202,7 +203,7 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
         dS = scale * P o (dO V^T - delta)              GEMM with a row bias (-scale * delta) and P as multiplicative operand
         dQ = dS K,  dK = dS^T Q,  dV = P^T dO          row contractions, operands consumed MN-major as stored
     with delta_t = sum_d dO_td O_td (`rowdot_heads`).  Round 1 materialised S and dP in fp32, ran a row softmax and its
-    backward over them and transposed dS / P / Q / K / dO with a gather kernel: ~125 of 254 ms of a bs-2 768^2 iteration.
+    backward over them and transposed dS / P / Q / K / dO with a gather kernel.
     Still materialises P and dS ([heads, T, Tk] fp16 per image): a fused flash backward would remove those too."""
     B, T, C = q.shape
     Tk = k.shape[1]

@@ -1,4 +1,4 @@
-"""Build libb200_e2eft.so (sm_100a only) in-tree with nvcc.  No torch dependency: the library is a
+"""Build libb200_e2eft.so (sm_90a only) in-tree with nvcc.  No torch dependency: the library is a
 plain C-ABI shared object (include/b200_e2eft.h) loaded through ctypes."""
 import hashlib
 import os
@@ -12,7 +12,7 @@ OUT = os.path.join(HERE, "libb200_e2eft.so")
 OBJ = os.path.join(HERE, "build")
 SOURCES = ["gemm_conv.cu", "attention.cu", "norm.cu", "elementwise.cu", "conv_small.cu", "loss.cu", "optim.cu", "backward.cu", "postproc.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC"]
 
 

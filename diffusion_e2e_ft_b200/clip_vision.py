@@ -8,7 +8,7 @@ cross-attention.  Parameter names are transformers' (`vision_model.embeddings.pa
 the GeoWizard checkpoint loads with `load_state_dict` / `from_pretrained`.
 
 Arithmetic (transformers==4.37.2 models/clip/modeling_clip.py, restated in oracle/clip_vision.py):
-patch embedding = one tcgen05 GEMM over the 14x14x3 patches (K 588 zero-padded to 640) whose epilogue adds the
+patch embedding = one wgmma GEMM over the 14x14x3 patches (K 588 zero-padded to 640) whose epilogue adds the
 position embedding and writes straight into rows 1.. of the token matrix; class token + its position row is a
 packed constant; pre-LayerNorm; N x the encoder layer of clip_text.py (non-causal: one flash-attention launch over
 the 257 tokens, head_dim 64; quick_gelu on the SiLU epilogue); post-LayerNorm of the class token; bias-free projection

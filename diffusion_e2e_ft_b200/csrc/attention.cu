@@ -1,32 +1,30 @@
-// Flash attention for head_dim 64 on sm_100a: softmax(Q K^T * scale) V, no mask.
+// Flash attention for head_dim 64 on sm_90a: softmax(Q K^T * scale) V, no mask.
 //
-// Warp-specialised, 256 query rows per CTA: warp0 = TMA producer (two Q tiles once, K/V tiles through
-// a 3-stage smem ring), warp1 = tcgen05 issuer, warps 2..5 / 6..9 = two softmax warpgroups, each
-// owning one 128-row query tile with one row per thread (the TMEM lane layout gives each thread its
-// own row, so row max / row sum need no shuffles).  The two warpgroups ping-pong: while one runs its
-// exp pass (the MUFU-bound part at head_dim 64) the tensor core serves the other one.  Per tile j and
-// warpgroup w:
-//   S = Q_w K_j^T        tcgen05.mma  M128 N128 K64   -> TMEM
-//   P = exp2(S*c - m*c)  fp32 in registers -> fp16 into smem (SWIZZLE_128B, K-major A operand)
-//   T = P V_j            tcgen05.mma  M128 N64  K128  -> TMEM; V consumed MN-major straight from its
-//                        [keys x d] TMA tile (no transpose)
-//   O = O*alpha + T      in registers (fp32), folded in while the next S is already available.
+// Warp-specialised, 192 query rows per CTA: warp 12 = TMA producer (the three Q tiles once, K/V tiles through a
+// 3-stage smem ring), warps 0..11 = three consumer warpgroups, each owning 64 query rows with S, P and O in registers.
+// Per key tile j and warpgroup w:
+//   S = Q_w K_j^T        wgmma m64n128k16 x 4, both operands from smem (K-major)  -> 64 fp32 registers per thread
+//   m, l, O *= alpha     online softmax; a row lives in the 4 lanes of a quad, so the row max / sum take 2 shuffles
+//   P = exp2(S*c - m*c)  fp16, repacked in registers straight into the A-operand fragment layout
+//   O += P V_j           wgmma m64n64k16 x 8, A = P from registers, V consumed MN-major from its [keys x d] TMA tile
+// The three warpgroups run independently; while one exponentiates, the tensor core serves the others.
 // Joint attention (GeoWizard): kv_segments = 2 walks the K/V tiles of batch b%(B/2) then
 // b%(B/2)+B/2 — the concatenated K/V of attention.py:482-491 is never materialised.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include "../../include/b200_e2eft.h"
 
 namespace b200 {
 
-constexpr int kAttThreads = 320;   // warp0 TMA, warp1 MMA, warps 2-5 softmax WG0, warps 6-9 softmax WG1
-constexpr int kBq = 128;           // query rows per softmax warpgroup (one row per thread)
-constexpr int kWG = 2;             // query tiles per CTA
-constexpr int kBk = 128;           // keys per tile
+constexpr int kAttWG = 3;                        // consumer warpgroups (query tiles) per CTA
+constexpr int kAttThreads = 128 * kAttWG + 32;   // + the TMA producer warp
+constexpr int kBq = 64;                          // query rows per warpgroup
+constexpr int kBk = 128;                         // keys per tile
 constexpr int kD = 64;
 constexpr int kKvStages = 3;
-constexpr int kTileBytes = kBk * kD * 2;      // 16 KB (Q, K, V tiles)
-constexpr int kPBytes = kBq * kBk * 2;        // 32 KB
-constexpr int kAttSmem = kWG * kTileBytes + kKvStages * 2 * kTileBytes + kWG * kPBytes + 1024 + 1024;
+constexpr int kQBytes = kBq * kD * 2;            // 8 KB
+constexpr int kKvBytes = kBk * kD * 2;           // 16 KB (K or V tile)
+constexpr int kAttSmem = kAttWG * kQBytes + kKvStages * 2 * kKvBytes + 1024 + 1024;
 
 struct AttParams {
   int B, heads, Lq, Lk, kv_segments;
@@ -54,31 +52,25 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   // the compiler keeps the shared address space (LDS/STS, no aliasing with global stores)
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;                                   // [kWG][16 KB]
-  uint8_t* sK = sQ + kWG * kTileBytes;                  // [stages][16 KB]
-  uint8_t* sV = sK + kKvStages * kTileBytes;
-  uint8_t* sP = sV + kKvStages * kTileBytes;            // [kWG][32 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + kWG * kPBytes);
+  uint8_t* sQ = smem;                                   // [kAttWG][8 KB]
+  uint8_t* sK = sQ + kAttWG * kQBytes;                  // [stages][16 KB]
+  uint8_t* sV = sK + kKvStages * kKvBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kKvStages * kKvBytes);
   uint64_t* q_full = bars;
   uint64_t* k_full = bars + 1;
   uint64_t* v_full = k_full + kKvStages;
   uint64_t* kv_empty = v_full + kKvStages;
-  uint64_t* s_full = kv_empty + kKvStages;              // [kWG][2]  S buffer filled by QK^T
-  uint64_t* o_full = s_full + 2 * kWG;                  // [kWG][2]  T = P V landed (aliases S buffer cols 0..63)
-  uint64_t* p_full = o_full + 2 * kWG;                  // [kWG]     P written, S buffer fully read
-  uint64_t* t_empty = p_full + kWG;                     // [kWG]     T folded into O -> its S buffer is reusable
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(t_empty + kWG);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (kWG * kBq);
+  const int q0 = blockIdx.x * (kAttWG * kBq);
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int tiles_per_seg = (p.Lk + kBk - 1) / kBk;
   const int n_tiles = tiles_per_seg * p.kv_segments;
   const int half_b = p.kv_segments == 2 ? p.B / 2 : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 * kAttWG && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
@@ -86,548 +78,145 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     for (int i = 0; i < kKvStages; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int i = 0; i < kWG; ++i) {
-      mbar_init(&s_full[2 * i], 1);
-      mbar_init(&s_full[2 * i + 1], 1);
-      mbar_init(&o_full[2 * i], 1);
-      mbar_init(&o_full[2 * i + 1], 1);
-      mbar_init(&p_full[i], kBq);
-      mbar_init(&t_empty[i], kBq);
+      mbar_init(&kv_empty[i], 128 * kAttWG);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  // TMEM: S[w][buf] at columns 256w + 128buf (+128); T_j = P_j V_j is written over columns 0..63 of the
-  // S buffer it was computed from (dead once P_j is in smem), so S can be double buffered within 512 columns
-  const uint32_t tS = tmem_base;
 
-  if (warp == 0) {
+  if (warp == 4 * kAttWG) {
     // ===================================================================== TMA producer
     if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, kWG * kTileBytes);
-      for (int w = 0; w < kWG; ++w)
-        tma_load_3d(&tmQ, q_full, sQ + w * kTileBytes, h * kD, q0 + w * kBq, b, kEvictFirst);
+      mbar_arrive_expect_tx(q_full, kAttWG * kQBytes);
+      for (int w = 0; w < kAttWG; ++w)
+        tma_load_3d(&tmQ, q_full, sQ + w * kQBytes, h * kD, q0 + w * kBq, b, kEvictFirst);
       int stage = 0;
       uint32_t phase = 0;
       for (int seg = 0; seg < p.kv_segments; ++seg) {
         const int kb = p.kv_segments == 2 ? (b % half_b) + seg * half_b : b;
         for (int j = 0; j < tiles_per_seg; ++j) {
           mbar_wait(&kv_empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&k_full[stage], kTileBytes);
-          tma_load_3d(&tmK, &k_full[stage], sK + stage * kTileBytes, h * kD, j * kBk, kb, kEvictLast);
-          mbar_arrive_expect_tx(&v_full[stage], kTileBytes);
-          tma_load_3d(&tmV, &v_full[stage], sV + stage * kTileBytes, h * kD, j * kBk, kb, kEvictLast);
+          mbar_arrive_expect_tx(&k_full[stage], kKvBytes);
+          tma_load_3d(&tmK, &k_full[stage], sK + stage * kKvBytes, h * kD, j * kBk, kb, kEvictLast);
+          mbar_arrive_expect_tx(&v_full[stage], kKvBytes);
+          tma_load_3d(&tmV, &v_full[stage], sV + stage * kKvBytes, h * kD, j * kBk, kb, kEvictLast);
           if (++stage == kKvStages) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================================================================== tcgen05 issuer
-    constexpr uint32_t idesc_qk = make_idesc_f16(kBq, kBk, 0, 0);
-    constexpr uint32_t idesc_pv = make_idesc_f16(kBq, kD, 0, 1);   // B (=V) is MN-major
-    mbar_wait(q_full, 0);
-    auto issue_qk = [&](int j, int w) {            // S[w][j&1] = Q[w] K_j^T
-      if (lane == 0) {
-        const int st = j % kKvStages;
-        const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + w * kTileBytes), 16, 1024);
-        const uint64_t kdesc = make_desc_sw128(smem_u32(sK + st * kTileBytes), 16, 1024);
+    return;
+  }
+  // ======================================================================= consumer warpgroups
+  const int w = warp >> 2;
+  // accumulator fragment: this thread holds rows r0 = 16 (warp & 3) + lane / 4 and r0 + 8 of the warpgroup's 64, columns
+  // 8 i + 2 (lane % 4) + {0, 1}: s[4i], s[4i+1] for row r0, s[4i+2], s[4i+3] for row r0 + 8
+  const int r0 = (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  float o[kD / 2];
 #pragma unroll
-        for (int k = 0; k < kD / 16; ++k)
-          umma_f16(tS + w * 256 + (j & 1) * kBk, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[2 * w + (j & 1)]);
-      }
-      __syncwarp();
-    };
-    mbar_wait(&k_full[0], 0);
-    tc_fence_after();
-    issue_qk(0, 0);
-    issue_qk(0, 1);
-    for (int j = 0; j < n_tiles; ++j) {
-      const int st = j % kKvStages;
-      // next S tiles first: they only need the buffer that held T_{j-1} to be drained
-      if (j + 1 < n_tiles) {
-        mbar_wait(&k_full[(j + 1) % kKvStages], ((j + 1) / kKvStages) & 1);
-        for (int w = 0; w < kWG; ++w) {
-          if (j >= 1) mbar_wait(&t_empty[w], (j - 1) & 1);
-          tc_fence_after();
-          issue_qk(j + 1, w);
-        }
-      }
-      for (int w = 0; w < kWG; ++w) {
-        mbar_wait(&p_full[w], j & 1);               // P[w](j) in smem, S[w][j&1] fully read by WG w
-        if (w == 0) mbar_wait(&v_full[st], (j / kKvStages) & 1);
-        tc_fence_after();
-        if (lane == 0) {
-          const uint32_t pbase = smem_u32(sP + w * kPBytes);
-          const uint32_t vbase = smem_u32(sV + st * kTileBytes);
-#pragma unroll
-          for (int k = 0; k < kBk / 16; ++k) {
-            // A = P[:, 16k..16k+16): K-major, two 64-key swizzle atoms of 16 KB each
-            const uint64_t pdesc = make_desc_sw128(pbase + (k >> 2) * (kBq * 128) + (k & 3) * 32, 16, 1024);
-            // B = V[16k..16k+16, :]: MN-major, 16 key rows = 2 groups of 8 rows (SBO = 1024 B)
-            const uint64_t vdesc = make_desc_sw128(vbase + k * 2048, 16, 1024);
-            umma_f16(tS + w * 256 + (j & 1) * kBk, pdesc, vdesc, idesc_pv, k != 0);
-          }
-          umma_commit(&o_full[2 * w + (j & 1)]);
-        }
-        __syncwarp();
-      }
-      if (lane == 0) umma_commit(&kv_empty[st]);     // K_j / V_j slot reusable once everything above retires
-      __syncwarp();
-    }
-  } else {
-    // ===================================================================== softmax warpgroups
-    const int w = (warp - 2) >> 2;                   // warpgroup: which 128-row query tile
-    const int quad = warp & 3;                       // TMEM lane quadrant of this warp
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const uint32_t ts_base = tS + w * 256 + lane_off;
-    float o[kD];
-#pragma unroll
-    for (int i = 0; i < kD; ++i) o[i] = 0.f;
-    float m = -INFINITY, l = 0.f, alpha_prev = 0.f;
-    const float c = p.scale_log2;
-    uint8_t* prow = sP + w * kPBytes + row * 128;
-    const int sw = row & 7;
+  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  const float c = p.scale_log2;
+  const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + w * kQBytes), 16, 1024);
+  mbar_wait(q_full, 0);
 
-    for (int j = 0; j < n_tiles; ++j) {
-      const int jj = j % tiles_per_seg;
-      const int valid = min(kBk, p.Lk - jj * kBk);
-      mbar_wait(&s_full[2 * w + (j & 1)], (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t ts = ts_base + (j & 1) * kBk;
-      // ---- pass 1: row max
-      float mx0 = -INFINITY, mx1 = -INFINITY;
-      if (valid == kBk) {
-#pragma unroll 1
-        for (int cc = 0; cc < kBk; cc += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(ts + cc, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            mx0 = fmaxf(mx0, __uint_as_float(r[e]));
-            mx1 = fmaxf(mx1, __uint_as_float(r[e + 1]));
-          }
-        }
-      } else {
-#pragma unroll 1
-        for (int cc = 0; cc < kBk; cc += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(ts + cc, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 32; ++e)
-            if (cc + e < valid) mx0 = fmaxf(mx0, __uint_as_float(r[e]));
-        }
-      }
-      const float m_new = fmaxf(m, fmaxf(mx0, mx1));
-      const float alpha = ex2_approx((m - m_new) * c);
-      const float mc = m_new * c;
-      // ---- fold the previous tile's P V product into O (T[w] must be drained before PV(j) is issued)
-      if (j > 0) {
-        mbar_wait(&o_full[2 * w + ((j - 1) & 1)], ((j - 1) >> 1) & 1);
-        tc_fence_after();
-        const uint32_t to = ts_base + ((j - 1) & 1) * kBk;
-#pragma unroll
-        for (int cc = 0; cc < kD; cc += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(to + cc, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 32; ++e) o[cc + e] = fmaf(o[cc + e], alpha_prev, __uint_as_float(r[e]));
-        }
-        tc_fence_before();
-        mbar_arrive(&t_empty[w]);        // the buffer that held S_{j-1} / T_{j-1} may take S_{j+1}
-      }
-      // ---- pass 2: P = exp2(S*c - m*c) -> fp16 smem (SWIZZLE_128B K-major A operand), row sum
-      float rs0 = 0.f, rs1 = 0.f;
-#pragma unroll 1
-      for (int cc = 0; cc < kBk; cc += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(ts + cc, r);
-        tmem_ld_wait();
-        uint8_t* pchunk = prow + (cc >> 6) * (kBq * 128);
-        if (valid == kBk) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i0 = g * 8 + e * 2;
-              const float p0 = ex2_approx(fmaf(__uint_as_float(r[i0]), c, -mc));
-              const float p1 = ex2_approx(fmaf(__uint_as_float(r[i0 + 1]), c, -mc));
-              rs0 += p0;
-              rs1 += p1;
-              pk[e] = pack_half2(p0, p1);
-            }
-            const int chunk16 = ((cc & 63) >> 3) + g;    // logical 16-byte chunk within the 128-B row
-            *reinterpret_cast<uint4*>(pchunk + ((chunk16 ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        } else {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint32_t pk[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int i0 = g * 8 + e * 2;
-              const float p0 = (cc + i0 < valid) ? ex2_approx(fmaf(__uint_as_float(r[i0]), c, -mc)) : 0.f;
-              const float p1 = (cc + i0 + 1 < valid) ? ex2_approx(fmaf(__uint_as_float(r[i0 + 1]), c, -mc)) : 0.f;
-              rs0 += p0;
-              rs1 += p1;
-              pk[e] = pack_half2(p0, p1);
-            }
-            const int chunk16 = ((cc & 63) >> 3) + g;
-            *reinterpret_cast<uint4*>(pchunk + ((chunk16 ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          }
-        }
-      }
-      l = fmaf(l, alpha, rs0 + rs1);
-      m = m_new;
-      alpha_prev = alpha;
-      tc_fence_before();          // our TMEM reads of S[w][j&1] are done before P V overwrites its first 64 columns
-      fence_proxy_async_smem();   // P visible to the tensor-core (async) proxy
-      mbar_arrive(&p_full[w]);
-    }
+  for (int j = 0; j < n_tiles; ++j) {
+    const int st = j % kKvStages;
+    const uint32_t ph = (j / kKvStages) & 1;
+    const int jj = j % tiles_per_seg;
+    const int valid = min(kBk, p.Lk - jj * kBk);
+    float s[kBk / 2];
+    mbar_wait(&k_full[st], ph);
     {
-      const int j = n_tiles - 1;
-      mbar_wait(&o_full[2 * w + (j & 1)], (j >> 1) & 1);
-      tc_fence_after();
-      const uint32_t to = ts_base + (j & 1) * kBk;
+      const uint64_t kdesc = make_desc_sw128(smem_u32(sK + st * kKvBytes), 16, 1024);
+      wgmma_fence();
 #pragma unroll
-      for (int cc = 0; cc < kD; cc += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(to + cc, r);
-        tmem_ld_wait();
+      for (int k = 0; k < kD / 16; ++k) wgmma_m64n128<0, 0>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands<kBk / 2>(s);
+    }
+    if (valid < kBk) {                               // ragged last key tile: columns >= valid do not exist
 #pragma unroll
-        for (int e = 0; e < 32; ++e) o[cc + e] = fmaf(o[cc + e], alpha_prev, __uint_as_float(r[e]));
+      for (int i = 0; i < kBk / 8; ++i) {
+        const int col = 8 * i + cq;
+        if (col >= valid) { s[4 * i] = -INFINITY; s[4 * i + 2] = -INFINITY; }
+        if (col + 1 >= valid) { s[4 * i + 1] = -INFINITY; s[4 * i + 3] = -INFINITY; }
       }
     }
-    const int qrow = q0 + w * kBq + row;
-    if (qrow < p.Lq && p.lse != nullptr)          // P_ij = exp2(S_ij * c - lse): what the backward pass recomputes P from
-      p.lse[((long long)b * p.heads + h) * p.Lq + qrow] = fmaf(m, c, log2f(l));
-    if (qrow < p.Lq) {
-      const float inv = 1.0f / l;
-      __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + h * kD;
+    float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int g = 0; g < kD; g += 8) {
-        uint4 u;
-        u.x = pack_half2(o[g] * inv, o[g + 1] * inv);
-        u.y = pack_half2(o[g + 2] * inv, o[g + 3] * inv);
-        u.z = pack_half2(o[g + 4] * inv, o[g + 5] * inv);
-        u.w = pack_half2(o[g + 6] * inv, o[g + 7] * inv);
-        *reinterpret_cast<uint4*>(dst + g) = u;
+    for (int i = 0; i < kBk / 8; ++i) {
+      mx[0] = fmaxf(mx[0], fmaxf(s[4 * i], s[4 * i + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(s[4 * i + 2], s[4 * i + 3]));
+    }
+    float alpha[2], mc[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      const float m_new = fmaxf(m[r], mx[r]);
+      alpha[r] = ex2_approx((m[r] - m_new) * c);     // m = -inf on the first tile -> 0
+      m[r] = m_new;
+      mc[r] = m_new * c;
+    }
+    // P = exp2(S c - m c) as fp16 A fragments: k-chunk kk (keys 16 kk .. 16 kk + 15) = accumulator columns 8 (2 kk) ..
+    uint32_t pa[kBk / 16][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int kk = 0; kk < kBk / 16; ++kk) {
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        const int i = 2 * kk + hf;
+        const float p0 = ex2_approx(fmaf(s[4 * i], c, -mc[0]));
+        const float p1 = ex2_approx(fmaf(s[4 * i + 1], c, -mc[0]));
+        const float p2 = ex2_approx(fmaf(s[4 * i + 2], c, -mc[1]));
+        const float p3 = ex2_approx(fmaf(s[4 * i + 3], c, -mc[1]));
+        rs[0] += p0 + p1;
+        rs[1] += p2 + p3;
+        pa[kk][2 * hf] = pack_half2(p0, p1);         // a0 / a2: row r0, a1 / a3: row r0 + 8
+        pa[kk][2 * hf + 1] = pack_half2(p2, p3);
       }
     }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l[r] = fmaf(l[r], alpha[r], rs[r]);
+#pragma unroll
+    for (int i = 0; i < kD / 8; ++i) {
+      o[4 * i] *= alpha[0];
+      o[4 * i + 1] *= alpha[0];
+      o[4 * i + 2] *= alpha[1];
+      o[4 * i + 3] *= alpha[1];
+    }
+    mbar_wait(&v_full[st], ph);
+    {
+      const uint32_t vbase = smem_u32(sV + st * kKvBytes);
+      wgmma_fence_operands<kD / 2>(o);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kBk / 16; ++kk)       // B = V[16 kk .. 16 kk + 15, :]: MN-major, 2 groups of 8 key rows
+        wgmma_m64n64_rs_bmn(o, pa[kk], make_desc_sw128(vbase + kk * 2048, 8192, 1024));
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_operands<kD / 2>(o);
+    }
+    mbar_arrive(&kv_empty[st]);                      // this warpgroup is done with K_j / V_j
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 1);
+    l[r] += __shfl_xor_sync(0xffffffffu, l[r], 2);
   }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// v3: S read ONCE.  Same warp roles, tiles and smem layout as the kernel above; what changes is where things live:
-//   * each softmax thread pulls its whole 128-column S row into registers with one tcgen05.ld round trip, releases the
-//     S buffer at once (the tensor core starts Q K_{j+1}^T while this tile is still being exponentiated) and runs row
-//     max, exp2 and the fp16 pack out of registers;
-//   * O stays in TMEM: P_j V_j accumulates onto it (tcgen05.mma accumulate), so there is no per-tile fold of a 64-column
-//     T back into registers.  When a row maximum grows the running O row would have to be multiplied by
-//     2^((m_old - m_new) c): that read-modify-write of O in TMEM is done lazily — only when some row of the warp has
-//     grown by more than 2^8 since its reference maximum was fixed (probabilities then stay <= 256, exact in fp32 sums
-//     and well inside fp16 for P); the normalisation by the row sum at the end absorbs the stale reference.
-// TMEM read traffic per tile and warp drops from 40 KB (S twice + T) to 16 KB and the ten exposed tcgen05.ld round trips
-// to one: 613-627 vs 590 TFLOP/s at B=8 h=5 L=9216 (profiles/attn_variants_r02.txt), the default since r2.
-// What did NOT help, measured on the same shape and removed again (same file): the two warpgroups taking turns in the
-// exp pass through named barriers (-2..-6 %: a lone warp per sub-partition cannot saturate the MUFU), two threads per
-// query row = 16 softmax warps (-2 %), a share of the exponentials as an FMA-pipe cubic (-4..-7 %), P V issued in two
-// 64-key halves so that the next tile never waits for it (-8 %).  Every variant lands on ~3000-3300 cycles per pair of
-// tiles; ncu of this kernel (profiles/ncu_r02_summary.txt): XU 60 %, issue 41 %, tensor 29 %, shared LSU 16 %, stalls led
-// by `wait` and `long_scoreboard` — a latency-bound serial chain per tile with two softmax warps per scheduler, not a
-// throughput limit.  Untried: P in TMEM (TS-mode MMA), two key tiles in flight per warpgroup.
-// TMEM columns per warpgroup w: S at 256 w, O at 256 w + 128.
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-         "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]),
-         "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]),
-         "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// tcgen05.wait::ld with the destination registers as in/out operands: the compiler cannot move their first use above it
-__device__ __forceinline__ void tmem_ld_wait_dep(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                 "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :: "memory");
-}
-
-constexpr float kLazyLog2 = 8.0f;      // rescale O only when a row maximum has grown by more than 2^8 (log2 domain)
-
-__global__ void __launch_bounds__(kAttThreads, 1)
-attention_d64_v3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                        const __grid_constant__ CUtensorMap tmV, const AttParams p) {
-  extern __shared__ __align__(16) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;                                   // [kWG][16 KB]
-  uint8_t* sK = sQ + kWG * kTileBytes;                  // [stages][16 KB]
-  uint8_t* sV = sK + kKvStages * kTileBytes;
-  uint8_t* sP = sV + kKvStages * kTileBytes;            // [kWG][32 KB]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + kWG * kPBytes);
-  uint64_t* q_full = bars;
-  uint64_t* k_full = bars + 1;
-  uint64_t* v_full = k_full + kKvStages;
-  uint64_t* kv_empty = v_full + kKvStages;
-  uint64_t* s_full = kv_empty + kKvStages;              // [kWG]  S = Q K_j^T landed in TMEM
-  uint64_t* s_empty = s_full + kWG;                     // [kWG]  S row copied to registers by all 128 threads
-  uint64_t* p_full = s_empty + kWG;                     // [kWG]  P_j in smem (and O rescaled if it had to be)
-  uint64_t* o_full = p_full + kWG;                      // [kWG]  P_j V_j accumulated: P smem reusable, O stable
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(o_full + kWG);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (kWG * kBq);
-  const int h = blockIdx.y;
-  const int b = blockIdx.z;
-  const int tiles_per_seg = (p.Lk + kBk - 1) / kBk;
-  const int n_tiles = tiles_per_seg * p.kv_segments;
-  const int half_b = p.kv_segments == 2 ? p.B / 2 : 0;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    mbar_init(q_full, 1);
-    for (int i = 0; i < kKvStages; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int i = 0; i < kWG; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&s_empty[i], kBq);
-      mbar_init(&p_full[i], kBq);
-      mbar_init(&o_full[i], 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-
-  if (warp == 0) {
-    // ===================================================================== TMA producer (as above)
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, kWG * kTileBytes);
-      for (int w = 0; w < kWG; ++w)
-        tma_load_3d(&tmQ, q_full, sQ + w * kTileBytes, h * kD, q0 + w * kBq, b, kEvictFirst);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int seg = 0; seg < p.kv_segments; ++seg) {
-        const int kb = p.kv_segments == 2 ? (b % half_b) + seg * half_b : b;
-        for (int j = 0; j < tiles_per_seg; ++j) {
-          mbar_wait(&kv_empty[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&k_full[stage], kTileBytes);
-          tma_load_3d(&tmK, &k_full[stage], sK + stage * kTileBytes, h * kD, j * kBk, kb, kEvictLast);
-          mbar_arrive_expect_tx(&v_full[stage], kTileBytes);
-          tma_load_3d(&tmV, &v_full[stage], sV + stage * kTileBytes, h * kD, j * kBk, kb, kEvictLast);
-          if (++stage == kKvStages) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================================================================== tcgen05 issuer
-    constexpr uint32_t idesc_qk = make_idesc_f16(kBq, kBk, 0, 0);
-    constexpr uint32_t idesc_pv = make_idesc_f16(kBq, kD, 0, 1);   // B (=V) is MN-major
-    if (lane == 0) {
-      auto issue_qk = [&](int j, int w) {            // S[w] = Q[w] K_j^T
-        const int st = j % kKvStages;
-        const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + w * kTileBytes), 16, 1024);
-        const uint64_t kdesc = make_desc_sw128(smem_u32(sK + st * kTileBytes), 16, 1024);
 #pragma unroll
-        for (int k = 0; k < kD / 16; ++k)
-          umma_f16(tmem_base + w * 256, qdesc + 2 * k, kdesc + 2 * k, idesc_qk, k != 0);
-        umma_commit(&s_full[w]);
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&k_full[0], 0);
-      tc_fence_after();
-      issue_qk(0, 0);
-      issue_qk(0, 1);
-      for (int j = 0; j < n_tiles; ++j) {
-        const int st = j % kKvStages;
-        // next S tiles first: S[w] is free as soon as warpgroup w holds its row of S_j in registers
-        if (j + 1 < n_tiles) {
-          mbar_wait(&k_full[(j + 1) % kKvStages], ((j + 1) / kKvStages) & 1);
-          for (int w = 0; w < kWG; ++w) {
-            mbar_wait(&s_empty[w], j & 1);
-            tc_fence_after();
-            issue_qk(j + 1, w);
-          }
-        }
-        for (int w = 0; w < kWG; ++w) {
-          mbar_wait(&p_full[w], j & 1);               // P[w](j) in smem, O[w] rescaled if needed
-          if (w == 0) mbar_wait(&v_full[st], (j / kKvStages) & 1);
-          tc_fence_after();
-          const uint32_t pbase = smem_u32(sP + w * kPBytes);
-          const uint32_t vbase = smem_u32(sV + st * kTileBytes);
+  for (int r = 0; r < 2; ++r) {
+    const int qrow = q0 + w * kBq + r0 + 8 * r;
+    if (qrow >= p.Lq) continue;
+    if (p.lse != nullptr && (lane & 3) == 0)       // P_ij = exp2(S_ij * c - lse): what the backward pass recomputes P from
+      p.lse[((long long)b * p.heads + h) * p.Lq + qrow] = fmaf(m[r], c, log2f(l[r]));
+    const float inv = 1.0f / l[r];
+    __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + h * kD + cq;
 #pragma unroll
-          for (int k = 0; k < kBk / 16; ++k) {
-            const uint64_t pdesc = make_desc_sw128(pbase + (k >> 2) * (kBq * 128) + (k & 3) * 32, 16, 1024);
-            const uint64_t vdesc = make_desc_sw128(vbase + k * 2048, 16, 1024);
-            umma_f16(tmem_base + w * 256 + 128, pdesc, vdesc, idesc_pv, (j | k) != 0);     // O[w] += P_j V_j
-          }
-          umma_commit(&o_full[w]);
-        }
-        umma_commit(&kv_empty[st]);                   // K_j / V_j slot reusable once everything above retires
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================================================================== softmax warpgroups
-    const int w = (warp - 2) >> 2;                   // warpgroup: which 128-row query tile
-    const int quad = warp & 3;                       // TMEM lane quadrant of this warp
-    const int row = quad * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(quad * 32) << 16;
-    const uint32_t t_s = tmem_base + w * 256 + lane_off;
-    const uint32_t t_o = t_s + 128;
-    float m = -INFINITY, l = 0.f;                    // m: the reference maximum the stored probabilities are relative to
-    const float c = p.scale_log2;
-    uint8_t* prow = sP + w * kPBytes + row * 128;
-    const int sw = row & 7;
-    for (int j = 0; j < n_tiles; ++j) {
-      const int jj = j % tiles_per_seg;
-      const int valid = min(kBk, p.Lk - jj * kBk);
-      mbar_wait(&s_full[w], j & 1);
-      tc_fence_after();
-      uint32_t s0[32], s1[32], s2[32], s3[32];       // this thread's S row, 128 columns
-      tmem_ld_32x32(t_s, s0);
-      tmem_ld_32x32(t_s + 32, s1);
-      tmem_ld_32x32(t_s + 64, s2);
-      tmem_ld_32x32(t_s + 96, s3);
-      tmem_ld_wait_dep(s0);
-      tmem_ld_wait_dep(s1);
-      tmem_ld_wait_dep(s2);
-      tmem_ld_wait_dep(s3);
-      tc_fence_before();
-      mbar_arrive(&s_empty[w]);                      // the tensor core may overwrite S[w] with Q K_{j+1}^T
-      if (valid < kBk) {                             // ragged last key tile: columns >= valid do not exist
-#pragma unroll
-        for (int e = 0; e < 32; ++e) {
-          if (e >= valid) s0[e] = 0xff800000u;
-          if (32 + e >= valid) s1[e] = 0xff800000u;
-          if (64 + e >= valid) s2[e] = 0xff800000u;
-          if (96 + e >= valid) s3[e] = 0xff800000u;
-        }
-      }
-      float mx0 = -INFINITY, mx1 = -INFINITY;
-#pragma unroll
-      for (int e = 0; e < 32; e += 2) {
-        mx0 = fmaxf(mx0, fmaxf(__uint_as_float(s0[e]), __uint_as_float(s1[e])));
-        mx1 = fmaxf(mx1, fmaxf(__uint_as_float(s0[e + 1]), __uint_as_float(s1[e + 1])));
-        mx0 = fmaxf(mx0, fmaxf(__uint_as_float(s2[e]), __uint_as_float(s3[e])));
-        mx1 = fmaxf(mx1, fmaxf(__uint_as_float(s2[e + 1]), __uint_as_float(s3[e + 1])));
-      }
-      const float m_new = fmaxf(m, fmaxf(mx0, mx1));
-      // lazy reference: keep m while the maximum has grown by <= 2^8 in the exponent domain (first tile: always adopt)
-      const bool adopt = (m_new - m) * c > kLazyLog2;            // m = -inf on the first tile -> +inf > 8 -> adopt
-      const float alpha = adopt ? ex2_approx((m - m_new) * c) : 1.0f;
-      if (adopt) m = m_new;
-      const float mc = m * c;
-      if (j > 0) {                                   // P V_{j-1} retired: the P buffer may be rewritten, O is stable
-        mbar_wait(&o_full[w], (j - 1) & 1);
-        tc_fence_after();
-      }
-      float rs0 = 0.f, rs1 = 0.f;
-      auto exp_chunk = [&](uint32_t (&r)[32], int cc) {           // 32 columns -> fp16 P in smem (SWIZZLE_128B, K-major)
-        uint8_t* pchunk = prow + (cc >> 6) * (kBq * 128);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint32_t pk[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e) {
-            const int i0 = g * 8 + e * 2;
-            const float p0 = ex2_approx(fmaf(__uint_as_float(r[i0]), c, -mc));
-            const float p1 = ex2_approx(fmaf(__uint_as_float(r[i0 + 1]), c, -mc));
-            rs0 += p0;
-            rs1 += p1;
-            pk[e] = pack_half2(p0, p1);
-          }
-          const int chunk16 = ((cc & 63) >> 3) + g;    // logical 16-byte chunk within the 128-B row
-          *reinterpret_cast<uint4*>(pchunk + ((chunk16 ^ sw) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-        }
-      };
-      exp_chunk(s0, 0);
-      exp_chunk(s1, 32);
-      exp_chunk(s2, 64);
-      exp_chunk(s3, 96);
-      l = fmaf(l, alpha, rs0 + rs1);
-      // O[w] row *= alpha where a reference maximum moved (warp-uniform decision: tcgen05.ld / st are warp-collective)
-      if (j > 0 && __any_sync(0xffffffffu, adopt)) {
-#pragma unroll
-        for (int cc = 0; cc < kD; cc += 32) {
-          uint32_t r[32];
-          tmem_ld_32x32(t_o + cc, r);
-          tmem_ld_wait_dep(r);
-#pragma unroll
-          for (int e = 0; e < 32; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) * alpha);
-          tmem_st_32x32(t_o + cc, r);
-        }
-        tmem_st_wait();
-      }
-      tc_fence_before();          // our TMEM accesses (S read, O rescale) are ordered before the tensor core's P V
-      fence_proxy_async_smem();   // P visible to the tensor-core (async) proxy
-      mbar_arrive(&p_full[w]);
-    }
-    mbar_wait(&o_full[w], (n_tiles - 1) & 1);
-    tc_fence_after();
-    const int qrow = q0 + w * kBq + row;
-    if (qrow < p.Lq && p.lse != nullptr)          // P_ij = exp2(S_ij * c - lse): what the backward pass recomputes P from
-      p.lse[((long long)b * p.heads + h) * p.Lq + qrow] = fmaf(m, c, log2f(l));
-    const float inv = 1.0f / l;
-    __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + h * kD;
-#pragma unroll
-    for (int cc = 0; cc < kD; cc += 32) {
-      uint32_t r[32];
-      tmem_ld_32x32(t_o + cc, r);
-      tmem_ld_wait_dep(r);
-      if (qrow < p.Lq) {
-#pragma unroll
-        for (int g = 0; g < 32; g += 8) {
-          uint4 u;
-          u.x = pack_half2(__uint_as_float(r[g]) * inv, __uint_as_float(r[g + 1]) * inv);
-          u.y = pack_half2(__uint_as_float(r[g + 2]) * inv, __uint_as_float(r[g + 3]) * inv);
-          u.z = pack_half2(__uint_as_float(r[g + 4]) * inv, __uint_as_float(r[g + 5]) * inv);
-          u.w = pack_half2(__uint_as_float(r[g + 6]) * inv, __uint_as_float(r[g + 7]) * inv);
-          *reinterpret_cast<uint4*>(dst + cc + g) = u;
-        }
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+    for (int i = 0; i < kD / 8; ++i)
+      *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_half2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
   }
 }
 
@@ -635,8 +224,6 @@ attention_d64_v3_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_co
 
 using namespace b200;
 
-static int g_att_version = 3;      // 3 = attention_d64_v3_kernel (S read once, O in TMEM), 2 = attention_d64_kernel
-extern "C" void b200_debug_set_attention_version(int v) { g_att_version = v; }
 
 extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls, const void* k,
                                   long long k_bs, long long k_ls, const void* v, long long v_bs,
@@ -653,6 +240,7 @@ extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
                  "b200_attention_d64: pointers must be 16-byte aligned");
   CUtensorMap tq, tk, tv;
   const uint32_t box[3] = {kD, kBq, 1};
+  const uint32_t kv_box[3] = {kD, kBk, 1};
   {
     uint64_t dims[3] = {(uint64_t)heads * kD, (uint64_t)Lq, (uint64_t)B};
     uint64_t str[2] = {(uint64_t)q_ls * 2, (uint64_t)q_bs * 2};
@@ -662,10 +250,10 @@ extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
   {
     uint64_t dims[3] = {(uint64_t)heads * kD, (uint64_t)Lk, (uint64_t)B};
     uint64_t str[2] = {(uint64_t)k_ls * 2, (uint64_t)k_bs * 2};
-    int r = encode_tmap(&tk, k, 3, dims, str, box, nullptr);
+    int r = encode_tmap(&tk, k, 3, dims, str, kv_box, nullptr);
     if (r) return r;
     uint64_t strv[2] = {(uint64_t)v_ls * 2, (uint64_t)v_bs * 2};
-    r = encode_tmap(&tv, v, 3, dims, strv, box, nullptr);
+    r = encode_tmap(&tv, v, 3, dims, strv, kv_box, nullptr);
     if (r) return r;
   }
   static bool configured_dev[kMaxDevices] = {false};      // per device: function attributes live in the context
@@ -673,8 +261,6 @@ extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
   bool& configured = configured_dev[dev_ < 0 ? 0 : dev_];
   if (!configured || dev_ < 0) {
     cudaError_t e = cudaFuncSetAttribute(attention_d64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttSmem);
-    if (e == cudaSuccess)
-      e = cudaFuncSetAttribute(attention_d64_v3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttSmem);
     if (e != cudaSuccess) {
       set_last_error("cudaFuncSetAttribute(attention smem=%d): %s", kAttSmem, cudaGetErrorString(e));
       return (int)e;
@@ -686,11 +272,8 @@ extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = (__half*)out; p.o_bs = o_bs; p.o_ls = o_ls;
   p.lse = lse;
-  dim3 grid((Lq + kWG * kBq - 1) / (kWG * kBq), heads, B);
-  if (g_att_version == 3)
-    attention_d64_v3_kernel<<<grid, kAttThreads, kAttSmem, (cudaStream_t)stream>>>(tq, tk, tv, p);
-  else
-    attention_d64_kernel<<<grid, kAttThreads, kAttSmem, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  dim3 grid((Lq + kAttWG * kBq - 1) / (kAttWG * kBq), heads, B);
+  attention_d64_kernel<<<grid, kAttThreads, kAttSmem, (cudaStream_t)stream>>>(tq, tk, tv, p);
   B200_CHECK_LAUNCH("attention_d64_kernel");
   return 0;
 }

@@ -1,7 +1,7 @@
 // Backward-pass kernels of the fine-tuning step (SURVEY.md §8 row a10; reference: training/train.py:545-566,
 // `accelerator.backward(loss)` through the UNet and the frozen VAE decoder).  Everything here is HBM-bound
 // streaming / reduction work; the GEMM-shaped halves of the backward pass (conv dgrad, conv/linear wgrad,
-// attention S/dP/dQ/dK/dV products) run on the tcgen05 kernels in gemm_conv.cu with re-packed or transposed
+// attention S/dP/dQ/dK/dV products) run on the wgmma kernels in gemm_conv.cu with re-packed or transposed
 // operands (backward_packing.py / backward.py).
 //
 //   gather_planar       NHWC -> [C][pixels] transpose with an optional tap shift / stride / nearest-2x source map:

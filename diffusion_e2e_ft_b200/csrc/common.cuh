@@ -1,5 +1,5 @@
-// Common sm_100a device helpers: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (MMA / TMEM),
-// UMMA descriptors.  Hand-written inline PTX — no CUTLASS/CuTe dependency.
+// Common sm_90a device helpers: mbarrier, TMA (cp.async.bulk.tensor), wgmma shared-memory
+// descriptors.  Hand-written inline PTX — no CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -51,7 +51,7 @@ __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (TMA / tcgen05.mma reads)
+  // order generic-proxy smem accesses before later async-proxy ones (TMA writes, wgmma reads)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
@@ -73,17 +73,15 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (error surfaces to the host) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (error surfaces to the host) instead of hanging the GPU.  No printf here: a
+// function call inside a kernel that issues wgmma makes ptxas serialise the whole wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
 #pragma unroll 1
   for (int i = 0; i < 64; ++i)
     if (mbar_try_wait(bar, parity)) return;           // fast path: no clock reads
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 8000000000LL) {  // ~4 s at 2 GHz
-      printf("b200: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 8000000000LL) __trap();      // ~4 s at 2 GHz
   }
 }
 
@@ -122,92 +120,22 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* m, uint64_t* bar,
       : "memory");
 }
 
-// ----------------------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc];  kind::f16 (fp16/bf16 in, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp receives lane (base_lane+i), cols [c, c+32)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor (64-bit), sm_100 format:
+// ----------------------------------------------------------------------------- wgmma descriptors
+// Shared-memory matrix descriptor (64-bit), sm_90 format:
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset>>4 [46,48) version = 1      [49,52) base offset = 0
-//   [61,64) layout: 0 none, 2 = SWIZZLE_128B, 4 = 64B, 6 = 32B
-// K-major SWIZZLE_128B tile (rows of 64 x 16-bit = 128 B, 8-row groups 1024 B apart):
-//   LBO unused (1), SBO = 1024.
+//   [32,46) stride-dim byte offset>>4 [49,52) base offset = 0      [62,64) layout: 1 = SWIZZLE_128B
+// K-major SWIZZLE_128B tile (rows of 64 x 16-bit = 128 B, 8-row groups 1024 B apart): LBO unused (16), SBO = 1024.
+// MN-major SWIZZLE_128B tile ([k-row][64 rows] atoms): LBO = byte distance of 64-row atoms, SBO = of 8-k-row groups.
+// The swizzle is a function of the absolute smem address, so a start address inside a 1024-byte atom (a k-step of
+// +32 B, or a whole 128-byte row further on) needs no base offset.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
                                                     uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
-}
-// Instruction descriptor for kind::f16: fp16 A/B, fp32 accumulate.
-//   [4,6) D fmt (1 = f32)  [7,10) A fmt (0 = f16, 1 = bf16)  [10,13) B fmt
-//   [15] A major (0 = K)   [16] B major (0 = K, 1 = MN)  [17,23) N>>3  [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn,
-                                                      uint32_t b_mn) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (a_mn << 15) | (b_mn << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------- host: tensor maps

@@ -1,6 +1,6 @@
 // 3x3 convolution (stride 1, pad 1) with a tiny number of output channels (Cout <= 8): the UNet / VAE
-// `conv_out` layers (320->4, 128->3, 512->8).  With N <= 8 the tcgen05 implicit GEMM is bound by
-// re-fetching every activation tile nine times through L2 (measured 4.2 ms per bs=8 768^2 step); this
+// `conv_out` layers (320->4, 128->3, 512->8).  With N <= 8 the wgmma implicit GEMM is bound by
+// re-fetching every activation tile nine times through L2; this
 // kernel stages a halo tile in shared memory once per 64-channel chunk and reuses it for all nine taps.
 // HBM-bound: reads the NHWC fp16 input exactly once, writes NCHW fp32.
 // Tensor work is negligible (N padded to 8) and runs on mma.sync m16n8k16 (fp16 in, fp32 accumulate).

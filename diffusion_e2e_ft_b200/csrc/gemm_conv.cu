@@ -1,4 +1,4 @@
-// Host side of the tcgen05 GEMM / implicit-GEMM conv: tensor-map construction, tile-shape
+// Host side of the wgmma GEMM / implicit-GEMM conv: tensor-map construction, tile-shape
 // selection, launch.  C-ABI entry points are declared in include/b200_e2eft.h.
 #include <cstdarg>
 #include <cstdio>
@@ -77,11 +77,11 @@ int current_device() {
 int sm_count() {
   static int n[kMaxDevices] = {0};          // immutable once written; a racing first call writes the same value
   const int dev = current_device();
-  if (dev < 0) return 148;
+  if (dev < 0) return 132;
   if (!n[dev]) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[dev] = v > 0 ? v : 148;
+    n[dev] = v > 0 ? v : 132;
   }
   return n[dev];
 }
@@ -149,9 +149,9 @@ static int launch_bn(int bn, bool swap, const CUtensorMap& a, const CUtensorMap&
   return -1;
 }
 
-// Per-k-block time of a 128 x n MMA tile in SM cycles: 2n tensor cycles (K=64), floored by the measured
-// ~365-cycle producer/issuer barrier round trip (profiles/README_r01.md).
-static double kblock_cycles(int n) { return n * 2.0 > 365.0 ? n * 2.0 : 365.0; }
+// Per-k-block time of a 128 x n MMA tile in SM cycles: 4n tensor cycles (K=64 at 2048 dense fp16 FMA per SM and
+// cycle), floored by a ~365-cycle producer / consumer barrier round trip per k-block (an estimate, not measured here).
+static double kblock_cycles(int n) { return n * 4.0 > 365.0 ? n * 4.0 : 365.0; }
 static double tiles_cost(long long tiles, int n) {
   long long waves = (tiles + sm_count() - 1) / sm_count();
   return (double)waves * (kblock_cycles(n) + 40.0);
@@ -164,7 +164,7 @@ static int g_halo_mode = 1;   // 1 = automatic (halo-resident patch for stride-1
 static int g_last_path = 0;   // 0 = per-tap boxes / GEMM, 1 = halo-resident conv (tests assert the path they mean to cover)
 
 // Tile geometry of the halo-resident conv: bh rows x bw columns of output pixels.  The per-tap MMA covers
-// N = round_up16((bw + 2) * bh) consecutive patch pixels (<= 256 accumulator columns), of which bw * bh are real outputs;
+// N = round_up64((bw + 2) * bh) consecutive patch pixels (one of the wgmma widths 64 / 128 / 192 / 256), of which bw * bh are real outputs;
 // the patch ((bh + 2) rows of bw + 2 pixels, plus the tail the last taps read past it) must fit kHaloMaxPatchPix rows.
 static bool pick_halo_tile(int Ho, int Wo, int* bw_out, int* bh_out) {
   double best = 0.0;
@@ -172,7 +172,7 @@ static bool pick_halo_tile(int Ho, int Wo, int* bw_out, int* bh_out) {
   for (int bw = 8; bw <= 254 && bw <= Wo; ++bw) {
     for (int bh = 1; bh <= 32 && bh <= Ho; ++bh) {
       const int pitch = bw + 2;
-      const int n = (pitch * bh + 15) / 16 * 16;
+      const int n = (pitch * bh + 63) / 64 * 64;
       if (n > 256) break;
       if ((bh + 2) * pitch + (n - pitch * bh) + 2 > kHaloMaxPatchPix) continue;
       const double ew = (double)Wo / ((double)((Wo + bw - 1) / bw) * bw);
@@ -197,7 +197,7 @@ extern "C" void b200_debug_set_flags(int f) { b200::g_debug = f; }
 extern "C" void b200_debug_set_swap(int m) { b200::g_swap_mode = m; }
 extern "C" void b200_debug_set_halo(int m) { b200::g_halo_mode = m; }
 extern "C" int b200_debug_last_path(void) { return b200::g_last_path; }
-extern "C" int b200_abi_version(void) { return 5; }
+extern "C" int b200_abi_version(void) { return 6; }
 // Tile width used by the GEGLU epilogue for a packed width N (= 2 x output width); weights must be
 // packed per tile as [value half | gate half] with this width.
 extern "C" int b200_geglu_block_n(int N) {
@@ -282,7 +282,7 @@ extern "C" int b200_linear(const void* A, long long lda, long long a_batch_strid
   {
     const uintptr_t omask = out_f32 ? 15 : 7;
     // linear layers: the transposing epilogue only pays off where it carries the fused statistics across tiles; for the
-    // small-K GEMMs of the transformer blocks the direct lane = channel stores are faster (r2 bench: 14.1 vs 16.8 ms / step)
+    // small-K GEMMs of the transformer blocks the direct lane = channel stores are cheaper
     p.vec_ok = swap && (chan_stats != nullptr || (g_debug & 128)) && !(g_debug & 64) && N % 4 == 0 && ldo % 4 == 0 &&
                out_batch_stride % 4 == 0 && ((uintptr_t)out & omask) == 0 &&
                (!residual || (ld_res % 4 == 0 && res_batch_stride % 4 == 0 && ((uintptr_t)residual & omask) == 0)) &&
@@ -375,7 +375,7 @@ extern "C" int b200_conv2d_nhwc(const void* X, int NB, int H, int W, int Cin, co
     int hbw = 0, hbh = 0;
     // epilogue-bound launches (fp32 output + fp32 residual over a short K = 9 * Cin <= 1152: 8 B read + 4-6 B written per
     // output element against ~1 us of MMA per tile) gain nothing from cheaper operand loads and lose ~10 % to the dead
-    // halo columns their epilogue still walks: r2 bench, 128->128 768^2 fp32: 740 (halo) vs 825 TFLOP/s (per-tap boxes)
+    // halo columns their epilogue still walks
     const bool epi_bound = out_f32 && residual && num_taps * Cin <= 1152 && !X2;
     const bool halo_vec = !(g_debug & 64) && (Cout % 4 == 0) && (!residual || ((uintptr_t)residual & 15) == 0) &&
                           (!out2_f16 || ((uintptr_t)out2_f16 & 7) == 0);      // the halo kernel has the vectorised epilogue only
@@ -383,7 +383,7 @@ extern "C" int b200_conv2d_nhwc(const void* X, int NB, int H, int W, int Cin, co
         pick_halo_tile(Ho, Wo, &hbw, &hbh)) {
       p.bw = hbw; p.bh = hbh;
       p.col_pitch = hbw + 2;
-      p.halo_n = ((hbw + 2) * hbh + 15) / 16 * 16;
+      p.halo_n = ((hbw + 2) * hbh + 63) / 64 * 64;
       p.tiles_w = (Wo + hbw - 1) / hbw;
       p.tiles_h = (Ho + hbh - 1) / hbh;
       p.m_tiles = NB * p.tiles_w * p.tiles_h;
@@ -452,7 +452,7 @@ extern "C" int b200_conv2d_nhwc(const void* X, int NB, int H, int W, int Cin, co
         if (g_force_bn && pc[i] != g_force_bn) continue;
         pick_patch(Ho, Wo, stride, pc[i], &bw, &bh);
         long long tiles = (long long)NB * ((Wo + bw - 1) / bw) * ((Ho + bh - 1) / bh) * ((Cout + 127) / 128);
-        double c = tiles_cost(tiles, pc[i]) * 0.85;   // measured: swapped tiles run ~20 % faster per FLOP
+        double c = tiles_cost(tiles, pc[i]) * 0.85;   // swapped tiles: cheaper epilogue, fewer barrier round trips
         if (c < best - 1e-9) { best = c; pix = pc[i]; swap = true; }
       }
     }

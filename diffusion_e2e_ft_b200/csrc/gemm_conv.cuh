@@ -1,6 +1,6 @@
-// tcgen05 GEMM + im2col-free implicit-GEMM convolution for sm_100a.
+// wgmma GEMM + im2col-free implicit-GEMM convolution for sm_90a.
 //
-//   D[M,N] = epilogue( A[M,K] * W[N,K]^T )        fp16 operands, fp32 accumulate in TMEM
+//   D[M,N] = epilogue( A[M,K] * W[N,K]^T )        fp16 operands, fp32 accumulate in registers
 //
 // * A/W tiles are staged by TMA (cp.async.bulk.tensor, SWIZZLE_128B) into a multi-stage smem ring.
 // * LINEAR mode: A is a 3-D tensor (K, rows, batch).
@@ -10,25 +10,26 @@
 //   out-of-bounds zero fill, the stride from the tensor map's element strides.  No im2col buffer.
 //   Optional second source A2 (same pixel tiling, 1x1) appends k-blocks: this fuses the
 //   ResnetBlock2D 1x1 `conv_shortcut` into conv2's accumulation.
-// * One elected thread issues tcgen05.mma (M=128, N=BLOCK_N, K=16); accumulators are double
-//   buffered in TMEM so the epilogue of tile i overlaps the main loop of tile i+1.
-// * Warp roles: warp0 = TMA producer, warp1 = MMA issuer (+TMEM alloc), warps 2..9 = epilogue: two warps
-//   per TMEM lane quadrant taking alternate 32-column chunks (the epilogue is latency-bound per warp).
+// * Two consumer warpgroups (warps 0-7) each issue wgmma m64nBLOCK_Nk16 for one 64-row half of the 128-row tile,
+//   accumulating in registers; warp 8 is the TMA producer.  After the main loop of a tile the accumulators are
+//   staged as fp32 into the (then idle) operand ring and the same 8 warps run the epilogue from there: thread
+//   (warp & 3, lane) owns accumulator row 32 (warp & 3) + lane, the two warps of a row quadrant take alternate
+//   32-column chunks.  The producer starts the next tile's loads once every epilogue thread has released the ring.
 // * Persistent: grid = min(#tiles, #SMs), static round-robin tile schedule (n fastest).
 #pragma once
 #include <type_traits>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace b200 {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;       // 64 x fp16 = one 128-byte swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kGemmThreads = 320;   // warp0 TMA, warp1 MMA, warps 2-9 epilogue (two per TMEM lane quadrant)
+constexpr int kMmaK = 16;
+constexpr int kGemmThreads = 288;   // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA producer
 constexpr int kEpiWarps = 8;
-constexpr int kAccStages = 2;
-constexpr int kAccStrideCols = 256;
+constexpr int kConsumerThreads = 32 * kEpiWarps;
 constexpr int kMaxTaps = 9;
 
 enum EpiAct { ACT_NONE = 0, ACT_SILU = 1, ACT_GEGLU = 2, ACT_GELU = 3, ACT_EXP2 = 4 };   // EXP2: P = exp2(alpha S - lse)
@@ -40,14 +41,14 @@ struct GemmParams {
   int act_mn, w_mn;            // LINEAR: the activation / weight operand is stored [K][rows] (MN-major, e.g. dY for a weight
                                // gradient dY^T X) and is fed to the MMA as is — no transposition pass.  smem layout per
                                // stage: rows / 64 boxes of [64 k-rows][64 rows x 2 B], 8192 B apart (descriptor LBO 8192,
-                               // SBO 1024: tools/micro/umma_mnmajor_test.cu)
+                               // SBO 1024)
   // ---- conv geometry (conv != 0)
   int conv;
   int Ho, Wo;                  // conv-output grid the M tiles walk over
   int bw, bh, tiles_w, tiles_h;
   int col_pitch;               // accumulator column q of a conv tile = pixel (q / col_pitch, q % col_pitch): bw normally,
                                // bw + 2 in halo mode (the two halo columns of every patch row ride along as dead columns)
-  int halo_n;                  // halo mode: N of the per-tap MMA = round_up16((bw + 2) * bh)
+  int halo_n;                  // halo mode: N of the per-tap MMA = round_up64((bw + 2) * bh)
   int cin_blocks, num_taps, in_stride;
   int tap_dy[kMaxTaps], tap_dx[kMaxTaps];
   int k2_blocks;               // trailing k-blocks read from A2 (1x1 shortcut)
@@ -79,10 +80,9 @@ struct GemmParams {
 constexpr int kSwapPitch = 36;      // floats per row of the swapped epilogue's transpose tile (16-byte aligned, conflict-free)
 
 // HALO (conv3x3, stride 1, swapped orientation): the activation patch of a tile — (bh+2) x (bw+2) pixels x 64 channels —
-// is loaded ONCE per 64-channel block and all nine taps are issued as row-shifted views of it (UMMA descriptors with a
+// is loaded ONCE per 64-channel block and all nine taps are issued as row-shifted views of it (wgmma descriptors with a
 // 128-byte-granular start address), instead of nine separate bw x bh boxes: 9x -> (bh+2)(bw+2)/(bh*bw) ~ 1.5x of
-// L2 -> smem activation traffic.  Measured motivation (profiles/conv_isolation_r02.txt): with the operand loads
-// removed the same MMA / epilogue schedule runs 1.5x faster (1047 -> 1567 TFLOP/s on the 128-ch 768^2 conv).
+// L2 -> smem activation traffic.
 constexpr int kHaloMaxPatchPix = 400;                       // (bw+2)*(bh+2) <= 400: 64x4, 96x2, 48x5, 32x8 tiles
 constexpr int kHaloPatchBytes = kHaloMaxPatchPix * 128;     // one 64-channel slab of the patch (50 KB, 1024-aligned)
 constexpr int kHaloWStages = 5;                             // 128 x 64 weight tiles in flight (16 KB each)
@@ -104,6 +104,11 @@ struct GemmSmem {
   static constexpr int kOperandBytes = HALO ? kHaloWStages * kABytes + 2 * kHaloPatchBytes : kStages * kStageBytes;
   static constexpr int kTotalBytes = kOperandBytes + kEpiBytes + kBarrierBytes + 1024;
   static_assert(kTotalBytes <= 227 * 1024, "shared memory budget");
+  // fp32 accumulator tile staged for the epilogue in the operand area; the odd-ish pitch keeps both the fragment
+  // stores (8 rows x 4 column pairs per warp) and the row reads (32 rows per warp) at <= 2-way bank conflicts
+  static constexpr int kAccPitch = BLOCK_N + 9;
+  static constexpr int kAccBytes = kBlockM * kAccPitch * 4;
+  static_assert(kAccBytes <= kOperandBytes, "the accumulator tile must fit the operand ring");
 };
 
 template <typename OutT>
@@ -159,19 +164,51 @@ __device__ __forceinline__ float gelu_erf_f(float x) {
   return 0.5f * x * (1.0f + erf_v);
 }
 
-// SWAP = false: accumulator rows (TMEM lanes) = 128 pixels, columns = BLOCK_N output channels.
+// CW consecutive staged accumulator values of one row
+template <int CW>
+__device__ __forceinline__ void acc_ld(const float* src, uint32_t (&r)[CW]) {
+#pragma unroll
+  for (int j = 0; j < CW; ++j) r[j] = __float_as_uint(src[j]);
+}
+
+// D (+)= A B^T for one 64-row half of the tile: wgmma m64nNk16 with the operand majorness as immediates
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_n(float* d, uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (N == 32) wgmma_m64n32<TA, TB>(d, da, db, scale_d);
+  else if constexpr (N == 64) wgmma_m64n64<TA, TB>(d, da, db, scale_d);
+  else if constexpr (N == 128) wgmma_m64n128<TA, TB>(d, da, db, scale_d);
+  else if constexpr (N == 160) wgmma_m64n160<TA, TB>(d, da, db, scale_d);
+  else if constexpr (N == 192) wgmma_m64n192<TA, TB>(d, da, db, scale_d);
+  else {
+    static_assert(N == 256, "tile width without a wgmma wrapper");
+    wgmma_m64n256<TA, TB>(d, da, db, scale_d);
+  }
+}
+template <int N>
+__device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, int scale_d, bool a_mn, bool b_mn) {
+  if (!a_mn && !b_mn) wgmma_n<N, 0, 0>(d, da, db, scale_d);
+  else if (!a_mn) wgmma_n<N, 0, 1>(d, da, db, scale_d);
+  else if (!b_mn) wgmma_n<N, 1, 0>(d, da, db, scale_d);
+  else wgmma_n<N, 1, 1>(d, da, db, scale_d);
+}
+// halo mode: N = halo_n (a multiple of 64, <= 256), both operands K-major
+__device__ __forceinline__ void wgmma_halo(float* d, uint64_t da, uint64_t db, int scale_d, int n) {
+  if (n <= 64) wgmma_n<64, 0, 0>(d, da, db, scale_d);
+  else if (n <= 128) wgmma_n<128, 0, 0>(d, da, db, scale_d);
+  else if (n <= 192) wgmma_n<192, 0, 0>(d, da, db, scale_d);
+  else wgmma_n<256, 0, 0>(d, da, db, scale_d);
+}
+
+// SWAP = false: accumulator rows = 128 pixels, columns = BLOCK_N output channels.
 // SWAP = true : operands swapped — rows = 128 output channels (weights are the M operand), columns =
 //               BLOCK_N pixels (activations are the N operand).  Used when Cout % 128 == 0: a 128-channel
 //               layer then issues 128x256 MMAs (half the operand smem traffic and half the per-k-block
-//               barrier round trips of 128x128), and since lanes = channels the NHWC stores of one
+//               barrier round trips of 128x128), and since rows = channels the NHWC stores of one
 //               accumulator column are contiguous — no smem transpose in the epilogue.
-// 320 threads = 10 warps, one CTA per SM: the busiest scheduler partition hosts three warps and owns 16384 registers,
-// i.e. 170 per thread — the 168 ptxas picks under these launch bounds is the hardware ceiling (a __maxnreg__(192) build
-// fails to launch), not a heuristic.
 // VEC (swapped orientation only): the vectorised epilogue (smem transpose, 16-byte accesses, statistics carried across
 // tiles) INSTEAD of the direct lane = channel one; a template parameter so that each instantiation carries one epilogue
-// only — with both compiled in, the small-K GEMMs of the transformer blocks (epilogue-bound) lost 25 % to spills and
-// instruction-cache misses (r2 bench: 14.1 -> 16.2 ms of linear GEMMs per step).
+// only — with both compiled in, the small-K GEMMs of the transformer blocks (epilogue-bound) lose time to spills and
+// instruction-cache misses.
 template <int BLOCK_N, typename OutT, bool SWAP, bool GEGLU, bool HALO = false, bool VEC = false>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmA2,
@@ -191,11 +228,10 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S::kOperandBytes + S::kEpiBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tmem_full = bars + 2 * kStages;
-  uint64_t* tmem_empty = bars + 2 * kStages + kAccStages;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 2 * kAccStages);
-  uint64_t* patch_full = bars + 2 * kStages + 2 * kAccStages + 1;      // HALO only
+  uint64_t* acc_empty = bars + 2 * kStages;            // every epilogue thread is done with the staged accumulators
+  uint64_t* patch_full = bars + 2 * kStages + 1;        // HALO only
   uint64_t* patch_empty = patch_full + 2;
+  float* acc_smem = reinterpret_cast<float*>(smem);     // [kBlockM][kAccPitch] fp32, in the operand ring between tiles
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -207,34 +243,28 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const uint32_t a_bytes = SWAP ? w_bytes : act_bytes;
   const uint32_t b_bytes = SWAP ? act_bytes : w_bytes;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kEpiWarps && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if (p.k2_blocks) tma_prefetch_desc(&tmA2);
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], kConsumerThreads);
     }
-    for (int i = 0; i < kAccStages; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], kEpiWarps);
-    }
+    mbar_init(acc_empty, kConsumerThreads);
     if constexpr (HALO) {
       for (int i = 0; i < 2; ++i) {
         mbar_init(&patch_full[i], 1);
-        mbar_init(&patch_empty[i], 1);
+        mbar_init(&patch_empty[i], kConsumerThreads);
       }
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp == kEpiWarps) {
     // ======================================================================= TMA producer
+    uint32_t aphase = 0;
     if constexpr (HALO) {
       if (lane == 0) {
         int ws = 0, pb = 0;
@@ -248,6 +278,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int th = r2 % p.tiles_h;
           const int img = r2 / p.tiles_h;
           const int h0 = th * p.bh, w0 = tw * p.bw;
+          mbar_wait(acc_empty, aphase ^ 1);                  // the accumulators of the previous tile left the ring
+          aphase ^= 1;
           for (int blk = 0; blk < p.cin_blocks + p.k2_blocks; ++blk) {
             const bool main = blk < p.cin_blocks;
             mbar_wait(&patch_empty[pb], pphase ^ 1);
@@ -293,6 +325,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           h0 = th * p.bh;
           w0 = tw * p.bw;
         }
+        mbar_wait(acc_empty, aphase ^ 1);                    // the accumulators of the previous tile left the ring
+        aphase ^= 1;
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], ((p.debug & 2) ? 0u : a_bytes) + ((p.debug & 4) ? 0u : b_bytes));
@@ -338,116 +372,133 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         }
       }
     }
-  } else if (warp == 1) {
-    // ======================================================================= MMA issuer
-    constexpr uint32_t idesc = make_idesc_f16(kBlockM, BLOCK_N, 0, 0);
-    if constexpr (HALO) {
-      if (lane == 0) {
-        int ws = 0, pb = 0, acc = 0;
-        uint32_t wphase = 0, pphase = 0, acc_phase = 0;
-        const uint32_t a_base = smem_u32(smem_a), patch_base = smem_u32(smem_b);
-        // One MMA per (tap, k-step): its N = halo_n accumulator columns are halo_n CONSECUTIVE patch pixels starting at
-        // (dy, dx), i.e. bh output rows of bw pixels with the two halo pixels of every patch row riding along as dead
-        // columns (masked in the epilogue).  N stays large (A = the 128 x 16 weight slice is fetched once per 208-256
-        // columns; with one MMA per output row, N = 64, the A re-reads made the kernel smem-bound: 730 vs 1047 TFLOP/s).
-        const uint32_t idesc_tap = make_idesc_f16(kBlockM, (uint32_t)p.halo_n, 0, 0);
-        const int pitch = p.bw + 2;
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-          mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * kAccStrideCols;
-          for (int blk = 0; blk < p.cin_blocks + p.k2_blocks; ++blk) {
-            const bool main = blk < p.cin_blocks;
-            mbar_wait(&patch_full[pb], pphase);
-            tc_fence_after();
-            const uint32_t pbase = patch_base + pb * kHaloPatchBytes;
-            const int ntaps = main ? p.num_taps : 1;
-            for (int t = 0; t < ntaps; ++t) {
-              // patch offsets (0..2) of tap t: any tap set inside the 3x3 neighbourhood, in any order (forward convs,
-              // flipped-tap data gradients, the 2x2 phases of nearest-2x + conv)
-              const int dy = main ? p.tap_dy[t] + 1 : 1, dx = main ? p.tap_dx[t] + 1 : 1;
-              mbar_wait(&full_bar[ws], wphase);
-              tc_fence_after();
-              const uint64_t adesc = make_desc_sw128(a_base + ws * S::kABytes, 16, 1024);
-              // B rows = patch pixels (dy * pitch + dx) ...: a 128-byte-granular start inside the SWIZZLE_128B tile.  The
-              // swizzle is a function of the absolute smem address, so the descriptor needs NO base offset
-              // (tools/micro/umma_rowoffset_test.cu on a B200: base-offset field 0 reads the named rows, (addr >> 7) & 7
-              // does not).
-              const uint64_t bdesc = make_desc_sw128(pbase + (uint32_t)((dy * pitch + dx) * 128), 16, 1024);
+  } else {
+    // ======================================================================= MMA + epilogue warpgroups
+    const int wg = warp >> 2;                        // MMA rows 64 wg .. 64 wg + 63 of the 128-row tile
+    int stage = 0, ws = 0, pb = 0;
+    uint32_t phase = 0, wphase = 0, pphase = 0;
+    // Main loop of this CTA's next tile; returns with the fp32 accumulators in acc_smem (row-major, kAccPitch).
+    // One k-block of MMAs stays in flight: a ring slot is released once the MMAs after it have been issued.
+    auto mma_tile = [&]() {
+      float d[BLOCK_N / 2];
 #pragma unroll
-              for (int k = 0; k < kBlockK / kUmmaK; ++k)
-                if (!(p.debug & 8)) umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc_tap, (blk | t | k) != 0);
-              umma_commit(&empty_bar[ws]);
-              if (++ws == kStages) { ws = 0; wphase ^= 1; }
+      for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
+      if constexpr (HALO) {
+        const uint32_t a_base = smem_u32(smem_a) + wg * 8192, patch_base = smem_u32(smem_b);
+        // One MMA per (tap, k-step): its N = halo_n accumulator columns are halo_n CONSECUTIVE patch pixels starting
+        // at (dy, dx), i.e. bh output rows of bw pixels with the two halo pixels of every patch row riding along as dead
+        // columns (masked in the epilogue).  N stays large: the weight slice is fetched once per 128-256 columns.
+        const int pitch = p.bw + 2;
+        int prev_ws = -1, prev_pb = -1;
+        for (int blk = 0; blk < p.cin_blocks + p.k2_blocks; ++blk) {
+          const bool main = blk < p.cin_blocks;
+          mbar_wait(&patch_full[pb], pphase);
+          const uint32_t pbase = patch_base + pb * kHaloPatchBytes;
+          const int ntaps = main ? p.num_taps : 1;
+          for (int t = 0; t < ntaps; ++t) {
+            // patch offsets (0..2) of tap t: any tap set inside the 3x3 neighbourhood, in any order (forward convs,
+            // flipped-tap data gradients, the 2x2 phases of nearest-2x + conv)
+            const int dy = main ? p.tap_dy[t] + 1 : 1, dx = main ? p.tap_dx[t] + 1 : 1;
+            mbar_wait(&full_bar[ws], wphase);
+            const uint64_t adesc = make_desc_sw128(a_base + ws * S::kABytes, 16, 1024);
+            // B rows = patch pixels (dy * pitch + dx) ...: a 128-byte-granular start inside the SWIZZLE_128B tile
+            const uint64_t bdesc = make_desc_sw128(pbase + (uint32_t)((dy * pitch + dx) * 128), 16, 1024);
+            wgmma_fence_operands<BLOCK_N / 2>(d);
+            wgmma_fence();
+            if (!(p.debug & 8)) {
+#pragma unroll
+              for (int k = 0; k < kBlockK / kMmaK; ++k)
+                wgmma_halo(d, adesc + 2 * k, bdesc + 2 * k, (blk | t | k) != 0, p.halo_n);
             }
-            umma_commit(&patch_empty[pb]);
-            pb ^= 1;
-            if (pb == 0) pphase ^= 1;
+            wgmma_commit();
+            wgmma_fence_operands<BLOCK_N / 2>(d);
+            wgmma_wait<1>();
+            if (prev_ws >= 0) mbar_arrive(&empty_bar[prev_ws]);
+            if (prev_pb >= 0) mbar_arrive(&patch_empty[prev_pb]);
+            prev_ws = ws;
+            prev_pb = t == ntaps - 1 ? pb : -1;
+            if (++ws == kStages) { ws = 0; wphase ^= 1; }
           }
-          umma_commit(&tmem_full[acc]);
-          if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+          pb ^= 1;
+          if (pb == 0) pphase ^= 1;
         }
-      }
-    } else
-    if (lane == 0) {            // a single thread runs the whole issue loop (no warp-wide polling / syncs)
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      const uint32_t a_base = smem_u32(smem_a), b_base = smem_u32(smem_b);
-      // MMA operand A = weights when SWAP, activations otherwise; either may be MN-major (stored [K][rows])
-      const bool a_mn = SWAP ? (p.w_mn != 0) : (p.act_mn != 0);
-      const bool b_mn = SWAP ? (p.act_mn != 0) : (p.w_mn != 0);
-      const uint32_t idesc_rt = make_idesc_f16(kBlockM, BLOCK_N, a_mn ? 1u : 0u, b_mn ? 1u : 0u);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccStrideCols;
+        wgmma_wait<0>();
+        wgmma_fence_operands<BLOCK_N / 2>(d);
+        mbar_arrive(&empty_bar[prev_ws]);
+        mbar_arrive(&patch_empty[prev_pb]);
+      } else {
+        const uint32_t a_base = smem_u32(smem_a) + wg * 8192, b_base = smem_u32(smem_b);
+        // MMA operand A = weights when SWAP, activations otherwise; either may be MN-major (stored [K][rows])
+        const bool a_mn = SWAP ? (p.w_mn != 0) : (p.act_mn != 0);
+        const bool b_mn = SWAP ? (p.act_mn != 0) : (p.w_mn != 0);
+        int prev = -1;
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
           mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
           // K-major: rows of 128 B, k-step = +32 B inside the swizzle row.  MN-major: [k-row][64 rows] atoms 8192 B apart
-          // (LBO), 8-k-row groups 1024 B apart (SBO), k-step = 16 k-rows = +2048 B.
-          const uint64_t adesc = a_mn ? make_desc_sw128(a_base + stage * S::kABytes, 8192, 1024)
-                                      : make_desc_sw128(a_base + stage * S::kABytes, 16, 1024);
-          const uint64_t bdesc = b_mn ? make_desc_sw128(b_base + stage * S::kBBytes, 8192, 1024)
-                                      : make_desc_sw128(b_base + stage * S::kBBytes, 16, 1024);
+          // (LBO), 8-k-row groups 1024 B apart (SBO), k-step = 16 k-rows = +2048 B.  Either way the 64-row half of this
+          // warpgroup starts 8192 B into the A tile.
+          const uint64_t adesc = make_desc_sw128(a_base + stage * S::kABytes, a_mn ? 8192 : 16, 1024);
+          const uint64_t bdesc = make_desc_sw128(b_base + stage * S::kBBytes, b_mn ? 8192 : 16, 1024);
           const uint64_t astep = a_mn ? 128 : 2, bstep = b_mn ? 128 : 2;        // in 16-byte units
+          wgmma_fence_operands<BLOCK_N / 2>(d);
+          wgmma_fence();
+          if (!(p.debug & 8)) {
 #pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            if (!(p.debug & 8)) umma_f16(d_tmem, adesc + astep * k, bdesc + bstep * k, idesc_rt, (kb | k) != 0);
+            for (int k = 0; k < kBlockK / kMmaK; ++k)
+              wgmma_tile<BLOCK_N>(d, adesc + astep * k, bdesc + bstep * k, (kb | k) != 0, a_mn, b_mn);
           }
-          umma_commit(&empty_bar[stage]);           // smem slot reusable once these MMAs retire
-          if (kb == p.num_k_blocks - 1) umma_commit(&tmem_full[acc]);
+          wgmma_commit();
+          wgmma_fence_operands<BLOCK_N / 2>(d);
+          wgmma_wait<1>();
+          if (prev >= 0) mbar_arrive(&empty_bar[prev]);
+          prev = stage;
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+        wgmma_wait<0>();
+        wgmma_fence_operands<BLOCK_N / 2>(d);
+        mbar_arrive(&empty_bar[prev]);
       }
-    }
-  } else {
-    // ======================================================================= epilogue (4 warps)
-    // TMEM gives each thread one accumulator ROW (32 consecutive columns per tcgen05.ld).  Writing that
+      // both warpgroups' MMAs have retired (they read the ring) before it is overwritten with the accumulators
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+      {
+        float* dst = acc_smem + (wg * 64 + (warp & 3) * 16 + (lane >> 2)) * S::kAccPitch + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          dst[8 * j] = d[4 * j];
+          dst[8 * j + 1] = d[4 * j + 1];
+          dst[8 * S::kAccPitch + 8 * j] = d[4 * j + 2];
+          dst[8 * S::kAccPitch + 8 * j + 1] = d[4 * j + 3];
+        }
+      }
+      asm volatile("bar.sync 1, 256;" ::: "memory");
+    };
+    // this thread's reads of the staged accumulators are done: the ring may take the next tile's TMA loads
+    auto release_acc = [&]() {
+      fence_proxy_async_smem();
+      mbar_arrive(acc_empty);
+    };
+    // Each thread reads one staged accumulator ROW (32 consecutive columns per chunk).  Writing that
     // straight to global memory touches 32 different 128-byte lines per store instruction, so every
     // 32x32 chunk is transposed through a padded smem tile first: afterwards lane = column, and each
     // residual load / output store of a row segment is one fully coalesced 128-byte (fp32) access.
-    const int quad = warp & 3;                       // TMEM lane quadrant this warp may access
+    const int quad = warp & 3;                       // row quadrant of the tile
     const int row_in_tile = quad * 32 + lane;
-    const int eg = (warp - 2) >> 2;                  // epilogue group: which half of the chunks
-    const int ew = warp - 2;                         // epilogue warp index 0..7
+    const int eg = warp >> 2;                        // epilogue group: which half of the chunks
+    const int ew = warp;                             // epilogue warp index 0..7
+    const float* t_row = acc_smem + row_in_tile * S::kAccPitch;
     if constexpr (SWAP) {
       // ------------------------------------------------------------------ swapped: lane = channel
       OutT* __restrict__ out = reinterpret_cast<OutT*>(p.out);
       const OutT* __restrict__ res = reinterpret_cast<const OutT*>(p.residual);
       const float* __restrict__ bias = p.bias;
       uint32_t* tab = reinterpret_cast<uint32_t*>(stage_smem);     // [2 acc][out|res][BLOCK_N] pixel offsets
-      const int et = threadIdx.x - 64;                             // 0..127 within the epilogue warps
-      int acc = 0;
-      uint32_t acc_phase = 0;
+      const int et = threadIdx.x;                                  // 0..255 within the epilogue warps
+      int acc = 0;                                                 // which of the two pixel-offset tables
       // Fused GroupNorm statistics of the vectorised path: per-lane shifted partial sums of this lane's four channels,
       // carried ACROSS the tiles this persistent CTA processes for the same (image, channel tile) and merged into the
       // global fp64 accumulators only when that key changes.  One atomic per tile and channel — tens of thousands of
-      // tiles hammering the same 2 x Cout addresses of an image — cost 0.3 ms per launch on the 768^2 convs
-      // (profiles/conv_stats_atomics_r02.txt); a CTA sees ~17 consecutive tiles of an image, so this is ~17x fewer.
+      // tiles hammering the same 2 x Cout addresses of an image — serialise on those addresses; a CTA sees many
+      // consecutive tiles of an image, so carrying the sums divides the atomics by that count.
       float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
       int scnt = 0;
       long long skey = -1;                                         // (image * N + first channel) the sums belong to
@@ -478,8 +529,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         scnt = 0;
       };
       // Vectorised path: the offsets of a tile's pixels RELATIVE to its first pixel are the same for every tile, so the
-      // table is built once per CTA (ncu r2: rebuilding it per tile — integer divisions, a 256-thread barrier — was 19 %
-      // of the epilogue's time); per tile only a 64-bit base and the (rows, columns) still inside the image change.
+      // table is built once per CTA (rebuilding it per tile costs integer divisions and a 256-thread barrier); per tile
+      // only a 64-bit base and the (rows, columns) still inside the image change.
       uint32_t* s_rel_out = tab;                                   // [BLOCK_N]
       uint32_t* s_rel_res = tab + BLOCK_N;                         // [BLOCK_N]
       uint32_t* s_dhdw = tab + 2 * BLOCK_N;                        // [BLOCK_N]  (dh << 16 | dw), dh = 0xFFFF: dead column
@@ -551,7 +602,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
         if constexpr (VEC) {
           // ---------------------------------------------------------------- vectorised path (16-byte accesses)
-          // TMEM hands each lane ONE channel of 32 pixels; NHWC wants, per pixel, runs of consecutive channels.  Each
+          // The staged row hands each lane ONE channel of 32 pixels; NHWC wants, per pixel, runs of consecutive channels.  Each
           // 32x32 chunk goes through a per-warp smem tile (STS.32 by pixel row, LDS.128 back): afterwards lane
           // (pr = lane / 8, q = lane % 8) owns channels 4q..4q+3 of pixels pr, pr+4, ..., pr+28, so residual loads /
           // output stores are 16-byte (fp32) or 8-byte (fp16) accesses, four 128-byte pixel rows per warp instruction
@@ -593,9 +644,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             if (cur_w != key_w && __any_sync(0xffffffffu, scnt > 0)) flush_stats();
             skey = key;
           }
-          mbar_wait(&tmem_full[acc], acc_phase);
-          tc_fence_after();
-          const uint32_t t_row = tmem_base + acc * kAccStrideCols + ((uint32_t)(quad * 32) << 16);
+          mma_tile();
           // conv tiles may use fewer than BLOCK_N accumulator columns (bw * bh pixels)
           const int ncols = p.conv ? min(BLOCK_N, (p.col_pitch * p.bh + 31) & ~31) : BLOCK_N;
           if (!(p.debug & 16)) {
@@ -609,14 +658,13 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 const bool ok = cq_ok && (int)(dd >> 16) < lim_h && (int)(dd & 0xFFFFu) < lim_w;
                 oo[i] = ok ? s_rel_out[c + 4 * i + pr] : 0xFFFFFFFFu;
               }
-              if (res_q != nullptr) {                // residual rows first: their latency hides behind the TMEM read
+              if (res_q != nullptr) {                // residual rows first: their latency hides behind the accumulator read
 #pragma unroll
                 for (int i = 0; i < 8; ++i)
                   if (oo[i] != 0xFFFFFFFFu) rres[i] = *reinterpret_cast<const Vec*>(res_q + s_rel_res[c + 4 * i + pr]);
               }
               uint32_t r[32];
-              tmem_ld_32x32(t_row + c, r);
-              tmem_ld_wait();
+              acc_ld(t_row + c, r);
 #pragma unroll
               for (int j = 0; j < 32; ++j) stgw[j * kSwapPitch + lane] = __uint_as_float(r[j]);
               __syncwarp();
@@ -643,9 +691,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                   for (int k = 0; k < 4; ++k) v[i][k] += r4[k];
                 }
               }
-              // phase B: activations, one contiguous block that a plain conv skips with a single branch (with the SiLU /
-              // GELU bodies interleaved into the unrolled pixel loop, 19 % of the epilogue's samples were instruction-
-              // fetch stalls: ncu r2)
+              // phase B: activations, one contiguous block that a plain conv skips with a single branch (SiLU / GELU bodies
+              // interleaved into the unrolled pixel loop bloat it with instruction-fetch stalls)
               if (p.act == ACT_SILU) {
 #pragma unroll
                 for (int i = 0; i < 8; ++i)
@@ -701,15 +748,11 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               __syncwarp();                          // the tile is rewritten by the next chunk
             }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-          if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+          release_acc();
+          acc ^= 1;
           continue;
         }
-        mbar_wait(&tmem_full[acc], acc_phase);
-        tc_fence_after();
-        const uint32_t t_row = tmem_base + acc * kAccStrideCols + ((uint32_t)(quad * 32) << 16);
+        mma_tile();
         if (!(p.debug & 16)) {
 #pragma unroll 1
           for (int c = eg * 32; c < BLOCK_N; c += 64) {
@@ -720,7 +763,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               roff[4 * q4] = t4.x; roff[4 * q4 + 1] = t4.y; roff[4 * q4 + 2] = t4.z; roff[4 * q4 + 3] = t4.w;
             }
             OutT rres[32];                 // kept in the storage type: converting right after each load would
-            if (res_b != nullptr) {        // serialise the loads (measured 2.3x slower for fp16 residuals)
+            if (res_b != nullptr) {        // serialise the loads
 #pragma unroll
               for (int q4 = 0; q4 < 8; ++q4) {
                 const uint4 t4 = reinterpret_cast<const uint4*>(t_res + c)[q4];
@@ -733,8 +776,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               }
             }
             uint32_t r[32];
-            tmem_ld_32x32(t_row + c, r);
-            tmem_ld_wait();
+            acc_ld(t_row + c, r);
             float vals[32];
 #pragma unroll
             for (int j = 0; j < 32; ++j) vals[j] = fmaf(__uint_as_float(r[j]), p.alpha, add);
@@ -792,10 +834,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           atomicAdd(dst, s1 + n * sh);
           atomicAdd(dst + 1, (double)st2 + 2.0 * sh * s1 + n * sh * sh);
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-        if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+        release_acc();
+        acc ^= 1;
       }
       if (VEC && p.chan_stats && __any_sync(0xffffffffu, scnt > 0)) flush_stats();
     } else {
@@ -805,8 +845,6 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     uint32_t* s_off_out = reinterpret_cast<uint32_t*>(rowmeta_smem + ew * 640);
     uint32_t* s_off_res = s_off_out + 32;
     float* s_bias_r = reinterpret_cast<float*>(s_off_res + 32);
-    int acc = 0;
-    uint32_t acc_phase = 0;
     OutT* __restrict__ out = reinterpret_cast<OutT*>(p.out);
     const OutT* __restrict__ res = reinterpret_cast<const OutT*>(p.residual);
     const float* __restrict__ bias = p.bias;
@@ -848,17 +886,14 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const OutT* __restrict__ res_b = res ? res + (long long)b * p.res_batch_stride : nullptr;
       __half* __restrict__ out2_b = p.out2 ? p.out2 + (long long)b * p.out_batch_stride : nullptr;
 
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t t_row = tmem_base + acc * kAccStrideCols + ((uint32_t)(quad * 32) << 16);
+      mma_tile();
 
       if (p.debug & 16) {
       } else if (p.out_nchw) {
         if (eg == 0) {
         // tiny Cout (<= 8): thread = pixel, consecutive lanes = consecutive pixels -> already coalesced
         uint32_t r[16];
-        tmem_ld_32x16(t_row, r);
-        tmem_ld_wait();
+        acc_ld(t_row, r);
         if (row_ok) {
           const long long plane = (long long)p.OH * p.OW;
 #pragma unroll
@@ -891,7 +926,7 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             roff[4 * q4] = t4.x; roff[4 * q4 + 1] = t4.y; roff[4 * q4 + 2] = t4.z; roff[4 * q4 + 3] = t4.w;
           }
           // residual rows for this chunk: 32 independent coalesced loads in flight per warp, issued
-          // before the TMEM load / transpose so their latency is hidden
+          // before the accumulator load / transpose so their latency is hidden
           OutT rres[geglu ? 1 : 32];
           if constexpr (!geglu) if (res_b != nullptr) {
 #pragma unroll
@@ -906,15 +941,13 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             }
           }
           uint32_t r[CW];
-          if constexpr (CW == 32) tmem_ld_32x32(t_row + c, r); else tmem_ld_32x16(t_row + c, r);
-          tmem_ld_wait();
+          acc_ld(t_row + c, r);
           float gact[geglu ? 32 : 1];
           if constexpr (geglu) {
             // gate half first: transpose it, add its bias and apply erf-GELU with lane = column (batched,
             // branch-free); the value half then goes through the normal transposed path below
             uint32_t g[CW];
-            if constexpr (CW == 32) tmem_ld_32x32(t_row + width + c, g); else tmem_ld_32x16(t_row + width + c, g);
-            tmem_ld_wait();
+            acc_ld(t_row + width + c, g);
 #pragma unroll
             for (int e = 0; e < CW; ++e) stg[lane][e] = __uint_as_float(g[e]);
             __syncwarp();
@@ -1003,20 +1036,9 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           else do_chunk(c, std::integral_constant<int, 16>{});
         }
       }
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-      if (++acc == kAccStages) { acc = 0; acc_phase ^= 1; }
+      release_acc();
     }
     }  // !SWAP
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -170,8 +170,7 @@ __global__ void gn_apply_kernel(const T* __restrict__ x1, int C1, const T* __res
   __half* rb = raw ? raw + (long long)n * HW * C + c0 : nullptr;
   // 8 pixels per iteration: eight independent 16/32-byte loads in flight per thread (latency-bound otherwise).  The
   // loaded vectors stay in their storage type until use (fp16 input: 4 registers per pixel instead of 8), which keeps
-  // the fp16 instantiation under 85 registers = three 256-thread CTAs per SM (ncu r2: 119 registers / 2 CTAs, 81 % of
-  // the HBM roofline).
+  // the fp16 instantiation under 85 registers = three 256-thread CTAs per SM instead of two.
   using Raw = typename std::conditional<sizeof(T) == 2, uint4, float4>::type;
   constexpr int kRawPerPix = sizeof(T) == 2 ? 1 : 2;
   auto unpack = [](const Raw* rv, float* f) {
@@ -234,8 +233,8 @@ static int gn_block(int C) {
 // ------------------------------------------------------------------------------ LayerNorm
 // one warp per row; C <= 2048, C % 8 == 0.  Two-pass in registers (exact mean, then variance).
 // NV = per-lane 8-element vectors actually needed (ceil(C / 256)) is a template parameter: with the fixed 8 (64 value
-// registers, most of them dead for C = 320 / 640) the kernel ran 2 CTAs per SM and kept ~20 KB in flight per SM — 29 %
-// of the HBM roofline (r2 bench: 1.96 ms / step for 3.7 GB).
+// registers, most of them dead for C = 320 / 640) the kernel runs 2 CTAs per SM and keeps too few bytes in flight to
+// approach the HBM roofline.
 template <typename T, int NV>
 __global__ void layer_norm_kernel(const T* __restrict__ x, long long rows, int C,
                                   const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -359,8 +358,8 @@ __global__ void softmax_rows_kernel(const float* __restrict__ S, long long lds, 
 // Same result, one HBM read per row: the fp32 row is staged in shared memory (cols <= 16384) and the max / sum / write
 // passes run out of it.  Persistent CTAs; the rows arrive by cp.async.bulk (one elected thread, no register staging)
 // into a two-deep ring, so the next row is in flight while this one is reduced and written — with register-staged
-// loads issued by the same threads that later do the exp / store passes the kernel kept ~35 KB in flight per SM and sat
-// at 59 % of the HBM roofline (r2 bench: 2.1 ms / step for the VAE's two 9216 x 9216 score matrices per image).
+// loads issued by the same threads that later do the exp / store passes the kernel keeps too few bytes in flight per SM
+// to approach the HBM roofline.
 __device__ __forceinline__ void bulk_load_row(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");

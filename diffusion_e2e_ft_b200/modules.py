@@ -1,5 +1,5 @@
 """Building blocks of the engine: diffusers-named parameter containers whose forward runs the
-sm_100a kernels of libb200_e2eft.so (via ops.py) on NHWC activations.
+sm_90a kernels of libb200_e2eft.so (via ops.py) on NHWC activations.
 
 Layout / precision contract inside the engine
   * activations are NHWC; GEMM/conv operands are fp16; accumulation fp32;

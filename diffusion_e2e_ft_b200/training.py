@@ -143,11 +143,9 @@ class FlatTrainer:
     bucket's SUM all-reduce is launched asynchronously (NCCL stream) the moment autograd has accumulated its last
     parameter, as accelerate's DDP does for the reference; the DEFAULT is `overlap=False` — all buckets are reduced in
     `step()` after backward — because on this engine overlap can be a large loss: the GEMM / conv kernels are persistent
-    with one 200 KB-smem CTA per SM, so while NCCL's channel CTAs occupy SMs a 148-CTA grid no longer fits in one wave
-    and the backward kernels take two.  Measured, bs 2 768^2 per rank: 2 x B200 (P2P ring) 515 ms / step with overlap vs
-    260 ms without, against 5.7 ms for the 3.46 GB all-reduce alone (604 GB/s bus bandwidth); 8 x B200 (NVLS, few
-    CTAs) 178 vs 182 ms with 7.3 ms alone (827 GB/s) — profiles/bench_r02_n2.json, bench_r02_n8.json.  Exposing 4 % of
-    the step is the safe choice at every N.  The 1/world_size of the average is folded into the optimizer kernel's
+    with one ~200 KB-smem CTA per SM, so while NCCL's channel CTAs occupy SMs a 132-CTA grid no longer fits in one wave
+    and the backward kernels take two.  Exposing the all-reduce of the 3.46 GB gradient buffer after backward is the
+    safe choice at every N.  The 1/world_size of the average is folded into the optimizer kernel's
     gradient multiplier (no extra pass over the 3.46 GB buffer).
 
     Mixed precision: backward GEMM operands are fp16, so the loss is multiplied by a loss scale held ON THE DEVICE

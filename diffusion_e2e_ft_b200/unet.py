@@ -218,7 +218,7 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
         return ops.linear(e, ep["wall"], ep["ball"], out_dtype=F32)                  # all 22 time_emb_proj at once
 
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, return_dict=True, **unused):
-        ops._need_cuda(sample)                                                      # sm_100a only, no CPU fallback
+        ops._need_cuda(sample)                                                      # sm_90a only, no CPU fallback
         if torch.is_grad_enabled() and (sample.requires_grad or any(p.requires_grad for p in self.parameters())):
             return self._forward_train(sample, timestep, encoder_hidden_states, class_labels, return_dict)
         cfg, sdt = self.config, self.stream_dtype

@@ -23,7 +23,7 @@ _DEFAULTS = dict(in_channels=3, out_channels=3, latent_channels=4,
 class VAEAttention(nn.Module):
     """Single-head mid-block attention (d = channels, 512 for SD): GN -> q,k,v Linear(+bias) ->
     softmax(QK^T/sqrt(C)) V -> out Linear -> + residual  (instantiated as unet_2d_blocks.py:589-601).
-    Unfused on the tcgen05 GEMM: S = QK^T (fp32), row softmax, O = P V^T^T; V^T comes directly out of
+    Unfused on the wgmma GEMM: S = QK^T (fp32), row softmax, O = P V^T^T; V^T comes directly out of
     a swapped-operand GEMM (bias along rows), so no transpose kernel is needed."""
 
     def __init__(self, ch, groups, eps=1e-6):
@@ -88,7 +88,7 @@ class _UpDecoderBlock(nn.Module):
 
 
 def _check_input(x, who):
-    ops._need_cuda(x)                                  # sm_100a only, no CPU fallback
+    ops._need_cuda(x)                                  # sm_90a only, no CPU fallback
     if torch.is_grad_enabled() and x.requires_grad:
         raise NotImplementedError(f"backward through {who} is not implemented yet; wrap in torch.no_grad()")
 

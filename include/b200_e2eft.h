@@ -1,11 +1,11 @@
-/* b200_e2eft.h — C ABI of the B200-native single-step denoising engine (libb200_e2eft.so).
+/* b200_e2eft.h — C ABI of the H100-native single-step denoising engine (libb200_e2eft.so).
  *
  * Drop-in boundary for the hot path named by BASELINE.json `north_star`:
  *   VAE.encode -> UNet2DConditionModel forward (t=999) -> x0 -> VAE.decode.
  * The reference (VisualComputingInstitute/diffusion-e2e-ft) is pure Python and has no FFI of its
  * own; every entry point below replaces the third-party library kernel (cuDNN / cuBLAS / xformers /
  * ATen) behind one leaf operator of the reference's model graph.  The citation after each
- * prototype is the reference call site (relative to /root/reference) the function serves.
+ * prototype is the reference call site (relative to the reference repository root) the function serves.
  *
  * Conventions
  *   - plain pointers and sizes only; all pointers are CUDA device pointers owned by the caller
@@ -15,7 +15,7 @@
  *     b200_last_error_string() describes the last failure on the calling thread;
  *   - activations are NHWC ("channels last") fp16 operands; the residual stream may be fp16 or fp32
  *     (`*_f32` flags); accumulation, normalisation statistics and softmax are always fp32;
- *   - there is no CPU fallback: without an sm_100a device every launch returns an error.
+ *   - there is no CPU fallback: without an sm_90a device every launch returns an error.
  */
 #ifndef B200_E2EFT_H_
 #define B200_E2EFT_H_
@@ -35,7 +35,7 @@ int b200_abi_version(void);
 #define B200_ACT_EXP2 4  /* exp2(alpha * acc + bias): softmax probabilities recomputed from the log-sum-exp */
 
 /* out[b][m][n] = act( alpha * sum_k A[b][m][k] * W[(b)][n][k] + bias + residual[b][m][n] )
- * tcgen05 GEMM, fp16 operands (K contiguous), fp32 accumulate in TMEM.
+ * wgmma GEMM, fp16 operands (K contiguous), fp32 accumulate in registers.
  * Replaces: nn.Linear of proj_in/proj_out (GeoWizard/geowizard/models/transformer_2d.py:152-155,
  * 214-217), to_q/to_k/to_v/to_out (attention.py:470-478,501), GEGLU proj + FF out
  * (attention.py:755,765), TimestepEmbedding / time_emb_proj / class_embedding
@@ -56,7 +56,7 @@ int b200_linear(const void* A, long long lda, long long a_batch_stride,
                 void* out2_f16 /* optional fp16 copy of `out` (same strides) for a following GEMM operand */,
                 int res_mul /* 1: out = act(alpha*acc + bias) * residual (GEGLU as gate GEMM + value GEMM) */,
                 int a_mn /* 1: A is stored [K][M] (row pitch lda >= M): out = A^T-as-stored x W^T without a transposition
-                            pass (MN-major UMMA operand).  Weight gradients dW = dY^T X, attention backward dK = dS^T Q */,
+                            pass (MN-major wgmma operand).  Weight gradients dW = dY^T X, attention backward dK = dS^T Q */,
                 int w_mn /* 1: W is stored [K][N] (row pitch ldw >= N): data gradients dX = dY W, dQ = dS K */,
                 long long bias_batch_stride /* bias_row with batch > 1: bias of batch b starts at bias + b * stride */,
                 void* stream);
@@ -66,7 +66,7 @@ int b200_linear(const void* A, long long lda, long long a_batch_stride,
 int b200_geglu_block_n(int N);
 
 /* Implicit-GEMM convolution on NHWC fp16 input, weights packed [Cout][tap][Cin] (+[C2] shortcut
- * columns), tcgen05 + TMA, no im2col buffer.  Tap t reads input pixel
+ * columns), wgmma + TMA, no im2col buffer.  Tap t reads input pixel
  * (ho*stride + tap_dy[t], wo*stride + tap_dx[t]); out-of-range pixels read as zero (padding).
  * Output pixel (ho,wo) is written at (ho*out_mul+out_oy, wo*out_mul+out_ox) of an
  * (Ho*out_mul x Wo*out_mul) NHWC (or NCHW when out_nchw) tensor.
@@ -277,7 +277,6 @@ void b200_debug_set_flags(int flags);
 /* 1 (default) = swap operands automatically when Cout % 128 == 0; 0 = never */
 void b200_debug_set_swap(int mode);
 void b200_debug_set_halo(int mode);   /* 1 = automatic halo-resident stride-1 3x3 conv (default), 0 = per-tap boxes */
-void b200_debug_set_attention_version(int v);      /* 2 = two-pass softmax, O in registers; 3 = S read once, O in TMEM */
 int b200_debug_last_path(void);       /* path of the last b200_conv2d_nhwc call: 1 = halo-resident, 0 = per-tap boxes */
 
 /* torchvision resize(x, size, BICUBIC, antialias=True) of [planes][H][W] fp32 (aten _upsample_bicubic2d_aa, Keys

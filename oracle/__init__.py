@@ -7,7 +7,7 @@ for the CUDA engine in `diffusion_e2e_ft_b200`.
 Only `tests/`, `__graft_entry__.smoke()` and `bench.py`'s CPU-baseline / `--impl reference`
 legs may import this package.  The product path never does.
 
-PARITY UNPINNED: the reference (`/root/reference`, pure Python) ships no tests, no golden
+PARITY UNPINNED: the reference (the reference checkout, pure Python) ships no tests, no golden
 vectors and no weights, and its arithmetic lives in `diffusers==0.30.2` /
 `xformers==0.0.24` (requirements.txt:2,8) which are not installable here (no network).
 The restatement follows the in-tree GeoWizard copies of the diffusers graph

@@ -3,7 +3,7 @@ per process for the empty prompt (Marigold/marigold/marigold_pipeline.py:355-369
 -> `self.text_encoder(text_input_ids)[0]` -> `empty_text_embed` [1, 2, 1024]).
 
 The implementation lives in a third-party dependency, transformers==4.37.2 (requirements.txt:7), absent from
-/root/reference: `models/clip/modeling_clip.py` — CLIPTextEmbeddings (token + learned position embedding),
+the reference checkout: `models/clip/modeling_clip.py` — CLIPTextEmbeddings (token + learned position embedding),
 CLIPEncoderLayer (pre-LN; causal multi-head self-attention with q scaled by head_dim**-0.5; MLP fc1 -> act -> fc2),
 final_layer_norm, pooled output = the hidden state at the EOS position.  Restated here from that published
 algorithm with the transformers `state_dict` names, and PINNED in tests/test_clip_text.py against the installed

@@ -3,7 +3,7 @@
 feature extractor's crop size, CLIP mean / std normalisation, `self.image_encoder(x).image_embeds.unsqueeze(1)`
 -> [1, 1, 768], once per input image).
 
-The model is transformers==4.37.2 (requirements.txt:7) `CLIPVisionModelWithProjection`, absent from /root/reference:
+The model is transformers==4.37.2 (requirements.txt:7) `CLIPVisionModelWithProjection`, absent from the reference checkout:
 models/clip/modeling_clip.py — CLIPVisionEmbeddings (bias-free patch conv, class token, learned positions),
 `pre_layrnorm` (sic), CLIPEncoderLayer x N (non-causal), `post_layernorm` of the class token, bias-free
 `visual_projection`.  Restated from that published algorithm with the transformers `state_dict` names and PINNED in

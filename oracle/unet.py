@@ -6,7 +6,7 @@ Follows the control flow of GeoWizard/geowizard/models/unet_2d_condition.py:845-
 :2374-2481 (UpBlock2D), transformer_2d.py:327-423 and attention.py:292-413,430-513,
 719-777.  Leaf ops (ResnetBlock2D, Downsample2D, Upsample2D, Attention, GEGLU,
 Timesteps, TimestepEmbedding) are third-party diffusers code that is NOT under
-/root/reference; they are restated from their published 0.30.2 semantics (SURVEY.md App. A).
+the reference checkout; they are restated from their published 0.30.2 semantics (SURVEY.md App. A).
 
 Parameter names reproduce the diffusers `state_dict` layout (SURVEY.md App. A.8).
 """

@@ -1,6 +1,6 @@
 """ORACLE (test infrastructure) — fp32 PyTorch restatement of the SD `AutoencoderKL`.
 
-The AutoencoderKL source (diffusers 0.30.2) is NOT under /root/reference; it is restated
+The AutoencoderKL source (diffusers 0.30.2) is NOT in the reference checkout; it is restated
 per SURVEY.md App. A.6.  Block shapes follow the in-tree GeoWizard copies:
 `DownEncoderBlock2D` unet_2d_blocks.py:1276-1333, `UNetMidBlock2D` :509-631 (attention
 instantiated at :589-601), `UpDecoderBlock2D` :2484-2541.  Call sites:

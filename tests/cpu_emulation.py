@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — plain-torch restatements of the contracts of the CUDA kernels behind
 `diffusion_e2e_ft_b200.ops` (include/b200_e2eft.h), installed over `ops` by CPU tests so the HOST-side logic that
 sequences the kernels (module wiring, saved tensors, operand re-packing of the backward pass) can be exercised
-without a GPU.  Never imported by the product; the kernels themselves are checked on the B200 (`-m gpu`)."""
+without a GPU.  Never imported by the product; the kernels themselves are checked on the GPU (`-m gpu`)."""
 import math
 
 import torch

@@ -1,5 +1,5 @@
-"""Generate tests/golden/reference_pins.pt by RUNNING THE REFERENCE'S OWN CODE (imported by path from
-/root/reference, read-only) on seeded inputs.  Only the reference files that import without diffusers can be
+"""Generate tests/golden/reference_pins.pt by RUNNING THE REFERENCE'S OWN CODE (imported by path from a checkout of
+VisualComputingInstitute/diffusion-e2e-ft, read-only) on seeded inputs.  Only the reference files that import without diffusers can be
 run here (VERDICT r1 weak #2):
 
     training/util/loss.py                        ScaleAndShiftInvariantLoss, AngularLoss   (+ autograd gradients)
@@ -10,10 +10,10 @@ run here (VERDICT r1 weak #2):
     Marigold/src/util/alignment.py               align_depth_least_square
 
 The UNet / VAE arithmetic itself lives in diffusers==0.30.2 (absent, not installable offline) and stays pinned only
-by the oracle restatement (SURVEY.md §8c).  /root/reference does not exist on the GPU box, so the outputs are
-committed as a small fixture and tests/test_reference_pins.py compares the oracle AND the CUDA kernels with it.
+by the oracle restatement (SURVEY.md §8c).  The outputs are committed as a small fixture, so the test suite needs no
+reference checkout: tests/test_reference_pins.py compares the oracle AND the CUDA kernels with it.
 
-    python tests/golden/make_reference_pins.py
+    python tests/golden/make_reference_pins.py <path to the reference checkout>
 """
 import importlib.util
 import os
@@ -22,7 +22,7 @@ import sys
 import numpy as np
 import torch
 
-REF = "/root/reference"
+REF = sys.argv[1] if len(sys.argv) > 1 else ""
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 
@@ -139,5 +139,5 @@ def main():
 
 if __name__ == "__main__":
     if not os.path.isdir(REF):
-        sys.exit("needs /root/reference (run in the build container, not on the GPU box)")
+        sys.exit("usage: make_reference_pins.py <path to the diffusion-e2e-ft reference checkout>")
     main()

@@ -189,7 +189,7 @@ def check_swap_epilogue_twins(seed=51):
 
 def check_conv_halo(NB=2, H=40, W=64, Cin=128, Cout=128, shortcut=0, residual=False, out_f32=False, rowvec=False,
                     stats=False, seed=71):
-    """Halo-resident stride-1 3x3 conv (one patch load per 64-channel block, nine taps as row-shifted UMMA views) vs
+    """Halo-resident stride-1 3x3 conv (one patch load per 64-channel block, nine taps as row-shifted wgmma views) vs
     torch AND vs the per-tap-box path of the same kernel; asserts that the halo path was really taken."""
     L = ops._lib.load()
     x = _rand(NB, H, W, Cin, seed=seed)
@@ -267,11 +267,17 @@ def check_conv_halo_taps(seed=91):
     return worst, 3e-5
 
 
-def check_attention_lse_and_rowdot(B=2, heads=5, Lq=300, Lk=200, seed=95):
+def check_attention_lse_and_rowdot(B=2, heads=5, Lq=300, Lk=200, seed=95, fused=False):
     """Flash kernel's log2-domain log-sum-exp output and the rowdot kernel (the two row statistics of the attention
-    backward) against torch; then P recomputed by the exp2-epilogue GEMM against softmax."""
+    backward) against torch; then P recomputed by the exp2-epilogue GEMM against softmax.  fused=True takes q from one
+    projection output and k, v as strided views of another."""
     C = heads * 64
-    q, k, v = _rand(B, Lq, C, seed=seed), _rand(B, Lk, C, seed=seed + 1), _rand(B, Lk, C, seed=seed + 2)
+    if fused:
+        q = _rand(B, Lq, 2 * C, seed=seed)[..., :C]
+        kv = _rand(B, Lk, 2 * C, seed=seed + 1)
+        k, v = kv[..., :C], kv[..., C:]
+    else:
+        q, k, v = _rand(B, Lq, C, seed=seed), _rand(B, Lk, C, seed=seed + 1), _rand(B, Lk, C, seed=seed + 2)
     scale = 64 ** -0.5
     o, lse = ops.attention_d64(q, k, v, heads, scale, want_lse=True)
     def split(t):
@@ -435,39 +441,25 @@ def check_softmax_rows(rows=300, cols=1152, seed=0):
 
 
 # ----------------------------------------------------------------------------------- attention
-def _attention_version(v):
-    from diffusion_e2e_ft_b200 import lib as _l
-    _l.load().b200_debug_set_attention_version(v)
-
-
-def with_attention_version(fn, version=2):
-    """Run an attention check on the other flash kernel: 3 (default) = attention_d64_v3_kernel (S read once, O accumulated
-    in TMEM, lazy rescale), 2 = the two-pass kernel with O in registers (kept selectable: b200_debug_set_attention_version)."""
-    def run():
-        _attention_version(version)
-        try:
-            return fn()
-        finally:
-            _attention_version(ATTENTION_DEFAULT_VERSION)
-    return run
-
-
-ATTENTION_DEFAULT_VERSION = 3
-
-
-def check_attention(B=2, heads=5, Lq=576, Lk=None, joint=False, gain=3.0, seed=0, ramp=None):
+def check_attention(B=2, heads=5, Lq=576, Lk=None, joint=False, gain=3.0, seed=0, ramp=None, separate=False):
+    """Flash kernel vs fp32 torch.  q, k, v are strided views of one fused projection output (the engine's layout);
+    separate=True passes them as three contiguous tensors instead (row strides C, not 3C / 2C)."""
     Lk = Lk or Lq
     C = heads * 64
     qkv = _rand(B, Lq, 3 * C, seed=seed)
-    if Lk == Lq:
+    if separate:
+        q = qkv[..., :C].contiguous()
+        kv = qkv if Lk == Lq else _rand(B, Lk, 2 * C, seed=seed + 1)
+        k, v = kv[..., -2 * C:-C].contiguous(), kv[..., -C:].contiguous()
+    elif Lk == Lq:
         q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
     else:
         q = qkv[..., :C]
         kv = _rand(B, Lk, 2 * C, seed=seed + 1)
         k, v = kv[..., :C], kv[..., C:]
     if ramp is not None:
-        # key magnitude grows (ramp > 0) or shrinks (< 0) along the sequence: the running row maximum keeps moving, by
-        # more AND by less than the lazy-rescale threshold of the v3 kernel (2^8), tile after tile
+        # key magnitude grows (ramp > 0) or shrinks (< 0) along the sequence: the running row maximum keeps moving tile
+        # after tile, so the online-softmax rescale of O and of the row sum is exercised
         r = torch.linspace(0.05, abs(ramp), Lk, device=DEV)
         r = r if ramp > 0 else r.flip(0)
         k = (k.float() * r[None, :, None]).half()
@@ -776,16 +768,18 @@ CHECKS = {
     "attn_lse_rowdot_exp2_gemm": check_attention_lse_and_rowdot,
     "attn_ramp_up": lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=6.0),
     "attn_ramp_down": lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=-6.0),
-    "attn_v2_self_576": with_attention_version(lambda: check_attention()),
-    "attn_v2_self_2304": with_attention_version(lambda: check_attention(B=1, heads=10, Lq=2304)),
-    "attn_v2_ragged_144": with_attention_version(lambda: check_attention(B=2, heads=20, Lq=144)),
-    "attn_v2_cross_2": with_attention_version(lambda: check_attention(Lq=576, Lk=2)),
-    "attn_v2_cross_77": with_attention_version(lambda: check_attention(Lq=300, Lk=77)),
-    "attn_v2_joint": with_attention_version(lambda: check_attention(B=4, heads=5, Lq=576, joint=True)),
-    "attn_v2_lse_rowdot_exp2_gemm": with_attention_version(check_attention_lse_and_rowdot),
-    "attn_v2_ramp_up": with_attention_version(lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=6.0)),
-    "attn_v2_ramp_down": with_attention_version(lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=-6.0)),
-    "attn_v2_single_query": with_attention_version(lambda: check_attention(B=2, heads=4, Lq=1, Lk=9)),
+    # attn_v2_*: the same shapes with the other operand layout (separate contiguous q / k / v; for the LSE check, strided
+    # views).  The name is kept from an earlier kernel variant of the same checks.
+    "attn_v2_self_576": lambda: check_attention(separate=True),
+    "attn_v2_self_2304": lambda: check_attention(B=1, heads=10, Lq=2304, separate=True),
+    "attn_v2_ragged_144": lambda: check_attention(B=2, heads=20, Lq=144, separate=True),
+    "attn_v2_cross_2": lambda: check_attention(Lq=576, Lk=2, separate=True),
+    "attn_v2_cross_77": lambda: check_attention(Lq=300, Lk=77, separate=True),
+    "attn_v2_joint": lambda: check_attention(B=4, heads=5, Lq=576, joint=True, separate=True),
+    "attn_v2_lse_rowdot_exp2_gemm": lambda: check_attention_lse_and_rowdot(fused=True),
+    "attn_v2_ramp_up": lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=6.0, separate=True),
+    "attn_v2_ramp_down": lambda: check_attention(B=1, heads=3, Lq=700, Lk=1500, ramp=-6.0, separate=True),
+    "attn_v2_single_query": lambda: check_attention(B=2, heads=4, Lq=1, Lk=9, separate=True),
     "upsample_2x": check_upsample,
     "upsample_size_f32": lambda: check_upsample(True, (15, 20)),
     "timestep_embedding": check_timestep_embedding,

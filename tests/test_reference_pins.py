@@ -2,15 +2,13 @@
 
 tests/golden/reference_pins.pt holds outputs of the reference's importable files — training/util/loss.py,
 training/util/unet_prep.py, GeoWizard/geowizard/utils/normal_ensemble.py, Marigold/marigold/util/ensemble.py,
-Marigold/src/util/{metric,alignment}.py — run on seeded inputs by tests/golden/make_reference_pins.py (committed; the
-GPU box has no /root/reference).  Here
-  * not gpu: the ORACLE restatements must reproduce them (and, when /root/reference is present, the reference files are
-    imported by path and compared live, so a stale fixture cannot hide drift);
+Marigold/src/util/{metric,alignment}.py — run on seeded inputs by tests/golden/make_reference_pins.py (committed, so that the suite needs no reference
+checkout).  Here
+  * not gpu: the ORACLE restatements must reproduce them;
   * gpu: the CUDA kernels (losses forward + backward, normals / depth ensembling, min-max, resize) must reproduce them.
 The UNet / VAE arithmetic itself lives in diffusers==0.30.2 (absent): it stays pinned by the oracle only (parity
 "partial" by rule, DESIGN.md §4).
 """
-import importlib.util
 import os
 import sys
 
@@ -24,7 +22,6 @@ from oracle import pipeline as OP  # noqa: E402
 from oracle.unet import replace_unet_conv_in  # noqa: E402
 
 PINS = os.path.join(HERE, "golden", "reference_pins.pt")
-REF = "/root/reference"
 
 
 @pytest.fixture(scope="module")
@@ -92,22 +89,6 @@ def test_oracle_metric_and_alignment_match_reference(pins):
     want = met["values"]["abs_relative_difference"]["full"]
     got = OP.abs_rel(met["pred"], met["gt"])
     assert abs(got.item() - want.item()) <= 1e-6 * want.item()
-
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="/root/reference only exists in the build container")
-def test_fixture_is_current_against_live_reference(pins):
-    """Re-run two of the reference functions live: the committed fixture must be what the reference produces now."""
-    def load(rel, name):
-        spec = importlib.util.spec_from_file_location(name, os.path.join(REF, rel))
-        mod = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(mod)
-        return mod
-    loss = load("training/util/loss.py", "ref_loss_live")
-    s = pins["ssi"]
-    assert torch.equal(loss.ScaleAndShiftInvariantLoss()(s["pred"], s["target"], s["mask"]), s["loss"])
-    nens = load("GeoWizard/geowizard/utils/normal_ensemble.py", "ref_nens_live")
-    for case in pins["ensemble_normals"].values():
-        assert torch.equal(nens.ensemble_normals(case["preds"]), case["out"])
 
 
 # ------------------------------------------------------------------------------------------------ CUDA vs reference

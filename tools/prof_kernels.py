@@ -14,8 +14,6 @@ if len(sys.argv) > 4:
     _l.load().b200_debug_force_block_n(int(sys.argv[4]))
 if len(sys.argv) > 5:
     _l.load().b200_debug_set_swap(int(sys.argv[5]))
-if os.environ.get("B200_ATT_VERSION"):
-    _l.load().b200_debug_set_attention_version(int(os.environ["B200_ATT_VERSION"]))
 if os.environ.get("B200_HALO"):
     _l.load().b200_debug_set_halo(int(os.environ["B200_HALO"]))
 dev = "cuda"
