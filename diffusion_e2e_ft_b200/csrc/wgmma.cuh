@@ -94,6 +94,12 @@ __device__ __forceinline__ void wgmma_m64n64_rs_bmn(float* d, const uint32_t (&a
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
 
+__device__ __forceinline__ void wgmma_m64n256_rs_bmn(float* d, const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {" WG_R0 "," WG_R8 "," WG_R16 "," WG_R24 "," WG_R32 "," WG_R40 "," WG_R48 "," WG_R56 "," WG_R64 "," WG_R72 "," WG_R80 "," WG_R88 "," WG_R96 "," WG_R104 "," WG_R112 "," WG_R120 "}, {%128, %129, %130, %131}, %132, 1, 1, 1, 1;"
+               : WG_D(0), WG_D(8), WG_D(16), WG_D(24), WG_D(32), WG_D(40), WG_D(48), WG_D(56), WG_D(64), WG_D(72), WG_D(80), WG_D(88), WG_D(96), WG_D(104), WG_D(112), WG_D(120)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
 #undef WG_R0
 #undef WG_R8
 #undef WG_R16

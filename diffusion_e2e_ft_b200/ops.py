@@ -340,6 +340,31 @@ def attention_d64(q, k, v, heads, scale, kv_segments=1, out=None, want_lse=False
     return (out, lse) if want_lse else out
 
 
+@_timed("attention")
+def attention_d512(q, k, v, scale, out=None):
+    """One head of width 512 (VAE mid-block): q [B,Lq,512], k/v [B,Lk,512] fp16 views (last dim contiguous, e.g.
+    slices of one fused [B, L, 1536] projection) -> fp16 [B,Lq,512].  Flash kernel: no L x L buffer."""
+    _need_cuda(q, k, v)
+    assert q.dtype == F16 and k.dtype == F16 and v.dtype == F16
+    assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
+    assert q.shape[-1] == 512 and k.shape[-1] == 512 and v.shape[-1] == 512
+    B, Lq = q.shape[0], q.shape[1]
+    Lk = k.shape[1]
+    assert k.shape[0] == B and v.shape[:2] == k.shape[:2]
+    if out is None:
+        out = torch.empty((B, Lq, 512), dtype=F16, device=q.device)
+    assert out.dtype == F16 and out.stride(-1) == 1 and tuple(out.shape) == (B, Lq, 512)
+    qb = q.stride(0) if B > 1 else q.stride(1) * Lq
+    kb = k.stride(0) if B > 1 else k.stride(1) * Lk
+    vb = v.stride(0) if B > 1 else v.stride(1) * Lk
+    ob = out.stride(0) if B > 1 else out.stride(1) * Lq
+    rc = _lib.load().b200_attention_d512(_p(q), qb, q.stride(1), _p(k), kb, k.stride(1), _p(v), vb, v.stride(1),
+                                         _p(out), ob, out.stride(1), B, Lq, Lk, float(scale), _stream())
+    _lib.check(rc, "b200_attention_d512")
+    STATS.add("attn", 4 * B * Lq * Lk * 512)
+    return out
+
+
 @_timed("bwd_misc")
 def rowdot_heads(a, c, heads):
     """delta[b, h, t] = sum_d a[b, t, h*64+d] * c[b, t, h*64+d]; a, c fp16 [B, L, >=heads*64] views -> fp32 [B, heads, L]."""

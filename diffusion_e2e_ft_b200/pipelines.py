@@ -84,6 +84,19 @@ class PipelineBase:
     def device(self):
         return next(self.unet.parameters()).device
 
+    # ---- diffusers' memory-efficient attention switch (Marigold/run.py:285), forwarded like DiffusionPipeline does
+    def enable_xformers_memory_efficient_attention(self, attention_op=None):
+        for k in self._module_names:
+            fn = getattr(getattr(self, k), "enable_xformers_memory_efficient_attention", None)
+            if fn is not None:
+                fn(attention_op)
+
+    def disable_xformers_memory_efficient_attention(self):
+        for k in self._module_names:
+            fn = getattr(getattr(self, k), "disable_xformers_memory_efficient_attention", None)
+            if fn is not None:
+                fn()
+
     @property
     def dtype(self):
         return next(self.unet.parameters()).dtype
@@ -169,12 +182,28 @@ def pyramid_noise_like(x, discount=0.9, generator=None):
     return noise / noise.std()
 
 
+def _check_image_size(H, W):
+    """The kernels index one image's activations with 32-bit unsigned element offsets; the largest is the VAE
+    decoder's 256-channel full-resolution tensor, so one image must stay under 2^32 / 256 pixels (16.7 MP)."""
+    if 256 * H * W >= 2 ** 32:
+        raise ValueError(f"a {W}x{H} input ({H * W / 1e6:.1f} MP) is over the engine's per-image limit of "
+                         f"{(2 ** 32 - 1) // 256 / 1e6:.1f} MP (256 * H * W < 2^32 elements); pass a "
+                         f"processing_res > 0 to run at a lower resolution")
+
+
+def _max_res_size(h, w, max_edge):
+    """(height, width) after resize_max_res; processing_res = 0 keeps the input size."""
+    if max_edge <= 0:
+        return h, w
+    s = min(max_edge / w, max_edge / h)
+    return int(h * s), int(w * s)
+
+
 def _resize_max_res(img, max_edge):
     """Marigold/marigold/util/image_util.py:79-108 resize_max_res: antialiased bilinear down-scale to a maximum edge
     length, on the device (csrc/postproc.cu)."""
     _, h, w = img.shape
-    s = min(max_edge / w, max_edge / h)
-    return resize_bilinear_aa(img, (int(h * s), int(w * s)))
+    return resize_bilinear_aa(img, _max_res_size(h, w, max_edge))
 
 
 class MarigoldPipeline(PipelineBase):
@@ -200,6 +229,7 @@ class MarigoldPipeline(PipelineBase):
             rgb = torch.from_numpy(np.asarray(input_image.convert("RGB")).copy()).permute(2, 0, 1)
         input_size = rgb.shape
         assert rgb.dim() == 3 and input_size[0] == 3, f"Wrong input shape {input_size}, expected [rgb, H, W]"
+        _check_image_size(*_max_res_size(input_size[-2], input_size[-1], processing_res))   # before any launch
         # pre-processing on the device (SURVEY.md §8 f2): the raw (uint8) image is uploaded once; resize + [0,255] ->
         # [-1,1] run as kernels (marigold_pipeline.py:237-247)
         was_u8 = rgb.dtype == torch.uint8
@@ -260,6 +290,7 @@ class MarigoldPipeline(PipelineBase):
         # the kernels index each tensor with 32-bit element offsets: split batches whose largest activation
         # (256 channels at full resolution in the VAE decoder) would exceed 2^32 elements
         B, _, H, W = rgb_in.shape
+        _check_image_size(H, W)
         max_b = max(1, (2 ** 32 - 1) // (256 * H * W))
         if B > max_b:
             return torch.cat([self.single_infer(rgb_in[i:i + max_b], num_inference_steps, show_pbar, noise=noise,
@@ -267,7 +298,8 @@ class MarigoldPipeline(PipelineBase):
                               for i in range(0, B, max_b)], dim=0)
         if (self.use_cuda_graph and noise == "zeros" and num_inference_steps == 1 and rgb_in.is_cuda
                 and not torch.cuda.is_current_stream_capturing()):
-            key = ("marigold", tuple(rgb_in.shape), rgb_in.dtype, bool(normals))
+            key = ("marigold", tuple(rgb_in.shape), rgb_in.dtype, bool(normals),
+                   bool(getattr(self.vae, "memory_efficient_attention", False)))
             return self._graphed(key, lambda x: self._single_infer_impl(x, 1, noise, normals, None), rgb_in)
         return self._single_infer_impl(rgb_in, num_inference_steps, noise, normals, generator)
 
@@ -375,6 +407,7 @@ class DepthNormalEstimationPipeline(PipelineBase):
                      noise="zeros", img_embed=None):
         device = input_rgb.device
         B = input_rgb.shape[0]
+        _check_image_size(input_rgb.shape[-2], input_rgb.shape[-1])
         self.scheduler.set_timesteps(num_inference_steps, device=device)
         if num_inference_steps != 1 or noise != "zeros":
             raise NotImplementedError("engine pipeline implements the E2E-FT setting: 1 step, zeros noise")
@@ -431,6 +464,7 @@ class DepthNormalEstimationPipeline(PipelineBase):
         else:
             rgb = torch.from_numpy(np.asarray(input_image.convert("RGB")).copy()).permute(2, 0, 1)
         input_size = rgb.shape
+        _check_image_size(*_max_res_size(input_size[-2], input_size[-1], processing_res))   # before any launch
         was_u8 = rgb.dtype == torch.uint8
         rgb = rgb.to(self.device).to(torch.float32)
         if processing_res > 0:

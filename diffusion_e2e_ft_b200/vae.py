@@ -20,11 +20,33 @@ _DEFAULTS = dict(in_channels=3, out_channels=3, latent_channels=4,
                  scaling_factor=0.18215, sample_size=768, act_fn="silu")
 
 
+# The unfused VAE attention stores S [B, L, Lp] fp32 and P fp16: 6 bytes per score.  Its GEMMs address one batch
+# element of an output with 32-bit offsets (b200_linear rejects M * ldo >= 2^32 - 1; for S that is L * Lp), while batch
+# offsets and the row softmax's offsets are 64-bit.  So the unfused path computes any batch size as long as one image's
+# score matrix stays under 2^32 - 1 elements, and that bound (not B * L * Lp) is where the fused kernel must take over:
+# every shape the unfused path can compute keeps it, bit for bit.
+UNFUSED_MAX_SCORES = 0xFFFFFFFF
+
+
+def use_fused_attention(B, L, ch, memory_efficient=False):
+    """Which path `VAEAttention.run` takes for B images of L = H*W tokens and `ch` channels: the d=512 flash kernel
+    (True) when memory-efficient attention is switched on or when the unfused path cannot index one image's scores;
+    otherwise the unfused GEMM + row-softmax path.  The flash kernel exists for 512 channels only (every reference
+    VAE); other widths always run unfused.  B does not enter: batch offsets are 64-bit on both paths."""
+    if ch != 512:
+        return False
+    Lp = (L + 7) // 8 * 8
+    return bool(memory_efficient) or L * Lp >= UNFUSED_MAX_SCORES
+
+
 class VAEAttention(nn.Module):
     """Single-head mid-block attention (d = channels, 512 for SD): GN -> q,k,v Linear(+bias) ->
     softmax(QK^T/sqrt(C)) V -> out Linear -> + residual  (instantiated as unet_2d_blocks.py:589-601).
-    Unfused on the wgmma GEMM: S = QK^T (fp32), row softmax, O = P V^T^T; V^T comes directly out of
-    a swapped-operand GEMM (bias along rows), so no transpose kernel is needed."""
+    Two paths (`use_fused_attention` picks one):
+      unfused (default): S = QK^T (fp32), row softmax, O = P V^T^T on the wgmma GEMM; V^T comes directly out of a
+        swapped-operand GEMM (bias along rows), so no transpose kernel is needed.  Needs 6 B per score (L^2 memory).
+      fused (`memory_efficient`, or L too large for the unfused path): one [B*L, 3C] QKV GEMM, the d=512 flash kernel
+        reading Q, K, V in place from it, then the same out-projection.  O(L) memory."""
 
     def __init__(self, ch, groups, eps=1e-6):
         super().__init__()
@@ -35,6 +57,7 @@ class VAEAttention(nn.Module):
         self.to_v = nn.Linear(ch, ch)
         self.to_out = nn.ModuleList([nn.Linear(ch, ch), nn.Dropout(0.0)])
         self._pk = Packed()
+        self.memory_efficient = False       # B200AutoencoderKL.enable_xformers_memory_efficient_attention
 
     def run(self, x, sdt=F32):
         pk = self._pk.get(list(self.parameters()), lambda: dict(
@@ -42,9 +65,18 @@ class VAEAttention(nn.Module):
             wqk=_f16(torch.cat([self.to_q.weight, self.to_k.weight], 0)),
             bqk=_f32(torch.cat([self.to_q.bias, self.to_k.bias], 0)),
             wv=_f16(self.to_v.weight), bv=_f32(self.to_v.bias),
+            wqkv=_f16(torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0)),
+            bqkv=_f32(torch.cat([self.to_q.bias, self.to_k.bias, self.to_v.bias], 0)),
             wo=_f16(self.to_out[0].weight), bo=_f32(self.to_out[0].bias)))
         B, H, W, C = x.shape
         L = H * W
+        if use_fused_attention(B, L, C, self.memory_efficient):
+            hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B * L, C)
+            qkv = ops.linear(hn, pk["wqkv"], pk["bqkv"]).view(B, L, 3 * C)
+            o = ops.attention_d512(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], C ** -0.5)   # [B, L, C]
+            out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt,
+                             stats_rows_per_img=L)
+            return _view_cs(out, B, H, W, C)
         Lp = (L + 7) // 8 * 8                       # leading dims must be multiples of 8 elements
         hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B, L, C)
         qk = ops.linear(hn.view(B * L, C), pk["wqk"], pk["bqk"]).view(B, L, 2 * C)
@@ -239,6 +271,26 @@ class B200AutoencoderKL(PretrainedMixin, nn.Module):
 
     def register_to_config(self, **kw):
         self.config.update({k: v for k, v in kw.items() if k in _DEFAULTS})
+
+    # ---- diffusers' memory-efficient attention switch (Marigold/run.py:285)
+    def enable_xformers_memory_efficient_attention(self, attention_op=None):
+        """Run both mid-block attentions (encoder and decoder) on the d=512 flash kernel, which never stores the
+        L x L score matrix: what makes native-resolution (`processing_res=0`) inference on large photos fit.
+        `attention_op` (an xformers operator in diffusers) is accepted and ignored: there is one kernel."""
+        self._set_memory_efficient_attention(True)
+
+    def disable_xformers_memory_efficient_attention(self):
+        """Back to the default: the unfused path wherever it can index the scores (see `use_fused_attention`)."""
+        self._set_memory_efficient_attention(False)
+
+    def _set_memory_efficient_attention(self, on):
+        for m in self.modules():
+            if isinstance(m, VAEAttention):
+                m.memory_efficient = bool(on)
+
+    @property
+    def memory_efficient_attention(self):
+        return any(m.memory_efficient for m in self.modules() if isinstance(m, VAEAttention))
 
     # ---- fused conveniences used by the engine's own pipelines (same math as the call sites above)
     def encode_scaled_mean(self, rgb):

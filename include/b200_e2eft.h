@@ -138,6 +138,20 @@ int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
                                      P_ij = exp2(scale * log2(e) * S_ij - lse_i) — the backward pass recomputes P from it */,
                        void* stream);
 
+/* Flash attention, one head of width 512 (the VAE mid-block), fp16 Q/K/V read in place from a
+ * (possibly fused) projection buffer: element (b, l, d) of Q is q[b*q_bs + l*q_ls + d] (same for K, V).
+ * out[b][l][d] = out[b*o_bs + l*o_ls + d] fp16.  softmax(QK^T*scale)V with fp32 scores and softmax
+ * statistics, fp16 P, fp32 accumulation; the L x L score matrix is never stored, so memory is O(L).
+ * Strides are multiples of 8 elements, row strides >= 512, pointers 16-byte aligned, 1 <= B <= 65535,
+ * Lq, Lk >= 1 (ragged lengths are fine).  No log-sum-exp output and no backward counterpart.
+ * Replaces the memory-efficient (xformers) attention of the VAE mid-block: unet_2d_blocks.py:589-601
+ * with `enable_xformers_memory_efficient_attention` (Marigold/run.py:285). */
+int b200_attention_d512(const void* q, long long q_bs, long long q_ls,
+                        const void* k, long long k_bs, long long k_ls,
+                        const void* v, long long v_bs, long long v_ls,
+                        void* out, long long o_bs, long long o_ls,
+                        int B, int Lq, int Lk, float scale, void* stream);
+
 /* Row softmax: P[r][:] = softmax(scale * S[r][:]) fp32 -> fp16 (VAE mid-block attention, d=512). */
 int b200_softmax_rows(const float* S, long long lds, void* P, long long ldp, long long rows,
                       int cols, float scale, void* stream);
