@@ -161,6 +161,41 @@ __global__ void decode_post_kernel(const float* __restrict__ x, long long HW, in
   }
 }
 
+// diffusers DDIMScheduler.step with eta = 0, in fp32 and in diffusers' order of operations (each product and sum
+// rounded on its own, no contraction): x0 / eps for the prediction type, then prev = sqrt(a_prev) x0 + sqrt(1-a_prev)
+// eps.  `prev` may alias `sample` (each element is read before it is written).  UI: 0 = no UNet-input copy, 1 = fp16,
+// 2 = fp32 copy of prev into a channel slice of the next UNet input.
+template <typename MO, int UI>
+__global__ void ddim_step_kernel(const MO* __restrict__ mo, long long mo_bs, const float* x, long long s_bs,
+                                 long long CHW, int ptype, float a_t, float a_prev, float* prev,
+                                 float* __restrict__ x0_out, void* __restrict__ ui, long long ui_bs) {
+  const int n = blockIdx.y;
+  const float beta = __fsub_rn(1.0f, a_t);
+  const float sa = sqrtf(a_t), sb = sqrtf(beta);
+  const float sp = sqrtf(a_prev), sd = sqrtf(__fsub_rn(1.0f, a_prev));
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < CHW;
+       i += (long long)gridDim.x * blockDim.x) {
+    const float m = (float)mo[n * mo_bs + i];
+    const float s = x ? x[n * s_bs + i] : 0.0f;
+    float x0, eps;
+    if (ptype == B200_PRED_V) {
+      x0 = __fsub_rn(__fmul_rn(sa, s), __fmul_rn(sb, m));
+      eps = __fadd_rn(__fmul_rn(sa, m), __fmul_rn(sb, s));
+    } else if (ptype == B200_PRED_EPSILON) {
+      x0 = __fdiv_rn(__fsub_rn(s, __fmul_rn(sb, m)), sa);
+      eps = m;
+    } else {                                                   // B200_PRED_SAMPLE
+      x0 = m;
+      eps = __fdiv_rn(__fsub_rn(s, __fmul_rn(sa, x0)), sb);
+    }
+    const float p = __fadd_rn(__fmul_rn(sp, x0), __fmul_rn(sd, eps));
+    prev[n * CHW + i] = p;
+    if (x0_out) x0_out[n * CHW + i] = x0;
+    if constexpr (UI == 1) reinterpret_cast<__half*>(ui)[n * ui_bs + i] = __float2half_rn(p);
+    if constexpr (UI == 2) reinterpret_cast<float*>(ui)[n * ui_bs + i] = p;
+  }
+}
+
 __global__ void cast_f32_f16_kernel(const float* __restrict__ x, __half* __restrict__ y, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x)
@@ -271,6 +306,39 @@ extern "C" int b200_decode_post(const float* x, int NB, long long HW, int mode, 
   dim3 grid(grid_for(HW, 256), NB);
   decode_post_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, HW, mode, sign, out);
   B200_CHECK_LAUNCH("decode_post_kernel");
+  return 0;
+}
+
+extern "C" int b200_ddim_step(const void* model_out, int mo_f16, long long mo_bstride, const float* sample,
+                              long long s_bstride, int B, int C, long long HW, int prediction_type,
+                              float alpha_prod_t, float alpha_prod_t_prev, float* prev_sample,
+                              float* pred_original_sample, void* unet_in, int unet_in_f16, long long ui_bstride,
+                              void* stream) {
+  B200_CHECK_ARG(model_out && prev_sample, "b200_ddim_step: null pointer");
+  B200_CHECK_ARG(B >= 1 && B <= 65535 && C >= 1 && HW >= 1, "b200_ddim_step: bad shape B=%d C=%d HW=%lld", B, C, HW);
+  const long long CHW = (long long)C * HW;
+  B200_CHECK_ARG(mo_bstride >= CHW && (!sample || s_bstride >= CHW) && (!unet_in || ui_bstride >= CHW),
+                 "b200_ddim_step: batch strides must be >= C*HW");
+  B200_CHECK_ARG((const void*)prev_sample != (const void*)sample || s_bstride == CHW,
+                 "b200_ddim_step: prev_sample may alias sample only when sample is contiguous (s_bstride = C*HW)");
+  B200_CHECK_ARG(prediction_type == B200_PRED_EPSILON || prediction_type == B200_PRED_V ||
+                 prediction_type == B200_PRED_SAMPLE, "b200_ddim_step: unknown prediction_type %d", prediction_type);
+  B200_CHECK_ARG(alpha_prod_t > 0.0f && alpha_prod_t < 1.0f && alpha_prod_t_prev >= 0.0f && alpha_prod_t_prev <= 1.0f,
+                 "b200_ddim_step: alpha_prod_t must be in (0, 1) and alpha_prod_t_prev in [0, 1]");
+  dim3 grid(grid_for(CHW, 256), B);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ui = unet_in ? (unet_in_f16 ? 1 : 2) : 0;
+#define B200_DDIM(MO, UI)                                                                                        \
+  ddim_step_kernel<MO, UI><<<grid, 256, 0, st>>>((const MO*)model_out, mo_bstride, sample, s_bstride, CHW,      \
+                                                 prediction_type, alpha_prod_t, alpha_prod_t_prev, prev_sample, \
+                                                 pred_original_sample, unet_in, ui_bstride)
+  if (mo_f16) {
+    if (ui == 0) B200_DDIM(__half, 0); else if (ui == 1) B200_DDIM(__half, 1); else B200_DDIM(__half, 2);
+  } else {
+    if (ui == 0) B200_DDIM(float, 0); else if (ui == 1) B200_DDIM(float, 1); else B200_DDIM(float, 2);
+  }
+#undef B200_DDIM
+  B200_CHECK_LAUNCH("ddim_step_kernel");
   return 0;
 }
 

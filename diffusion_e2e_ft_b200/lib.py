@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 7          # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 8          # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -49,6 +49,8 @@ _SIGS = {
     "b200_embed_tokens": (c_int, [_P, _P, _P, c_int, _LL, c_int, c_int, c_int, _P, _P]),
     "b200_pointwise_nchw": (c_int, [_P, c_float, _P, c_float, c_int, _P, _P, c_int, c_int, c_int, _LL, _P, _P]),
     "b200_decode_post": (c_int, [_P, c_int, _LL, c_int, c_float, _P, _P]),
+    "b200_ddim_step": (c_int, [_P, c_int, _LL, _P, _LL, c_int, c_int, _LL, c_int, c_float, c_float, _P, _P, _P, c_int,
+                               _LL, _P]),
     "b200_ssi_loss": (c_int, [_P, _P, _P, c_int, _LL, _P, _P, _P]),
     "b200_angular_loss": (c_int, [_P, _P, _P, c_int, _LL, _P, _P, _P]),
     "b200_sumsq": (c_int, [_P, _LL, _P, _P]),

@@ -455,6 +455,42 @@ def pointwise_nchw(in1, a1, wm, bias, in2=None, a2=0.0, cin=None):
     return out
 
 
+PREDICTION_TYPES = {"epsilon": 0, "v_prediction": 1, "sample": 2}      # B200_PRED_* of include/b200_e2eft.h
+
+
+def _nchw_inner_contiguous(t):
+    _, C, H, W = t.shape
+    return t.stride(3) == 1 and t.stride(2) == W and t.stride(1) == H * W
+
+
+@_timed("misc")
+def ddim_step(model_out, sample, alpha_prod_t, alpha_prod_t_prev, prediction_type="v_prediction", out=None,
+              want_x0=False, unet_in=None):
+    """DDIM update with eta = 0 (diffusers DDIMScheduler.step) -> (prev_sample fp32, pred_original_sample fp32 or None).
+    model_out [B,C,H,W] fp16/fp32 and sample (fp32, None = exact zeros) may be batch-strided; `out` (fp32, contiguous)
+    may be `sample` itself.  `unet_in`: a [B,C,H,W] fp16/fp32 view (e.g. channels 4..7 of the next UNet input) that
+    also receives prev_sample cast to its dtype."""
+    if prediction_type not in PREDICTION_TYPES:
+        raise ValueError(f"prediction_type {prediction_type!r} is not one of {sorted(PREDICTION_TYPES)}")
+    _need_cuda(model_out, sample, out, unet_in)
+    assert model_out.dim() == 4 and model_out.dtype in (F16, F32) and _nchw_inner_contiguous(model_out)
+    B, C, H, W = model_out.shape
+    if sample is not None:
+        assert sample.shape == model_out.shape and sample.dtype == F32 and _nchw_inner_contiguous(sample)
+    if out is None:
+        out = torch.empty((B, C, H, W), dtype=F32, device=model_out.device)
+    assert out.shape == model_out.shape and out.dtype == F32 and out.is_contiguous()
+    x0 = torch.empty((B, C, H, W), dtype=F32, device=model_out.device) if want_x0 else None
+    if unet_in is not None:
+        assert unet_in.shape == model_out.shape and unet_in.dtype in (F16, F32) and _nchw_inner_contiguous(unet_in)
+    _ck(_lib.load().b200_ddim_step(_p(model_out), int(model_out.dtype == F16), model_out.stride(0), _p(sample),
+                                   sample.stride(0) if sample is not None else 0, B, C, H * W,
+                                   PREDICTION_TYPES[prediction_type], float(alpha_prod_t), float(alpha_prod_t_prev),
+                                   _p(out), _p(x0), _p(unet_in), int(unet_in is not None and unet_in.dtype == F16),
+                                   unet_in.stride(0) if unet_in is not None else 0, _stream()), "b200_ddim_step")
+    return out, x0
+
+
 @_timed("misc")
 def decode_post(x, normals=False, sign=1.0, training=False):
     """`training`: the train.py:532-540 variants (no (x+1)/2 map for depth; clamp after normalising)."""

@@ -7,9 +7,12 @@ output dataclasses — and route the arithmetic through B200UNet2DConditionModel
 
   MarigoldPipeline                 <- Marigold/marigold/marigold_pipeline.py:113-538
   DepthNormalEstimationPipeline    <- GeoWizard/geowizard/models/geowizard_pipeline.py:67-401
-  DDIMScheduler (1-step closed form) <- diffusers DDIMScheduler as used at marigold_pipeline.py:401-402,457-465
+  DDIMScheduler (eta = 0, step on the b200_ddim_step kernel) <- diffusers DDIMScheduler as used at
+                                   marigold_pipeline.py:401-402,457-465 and geowizard_pipeline.py:261,326-334
 """
+import json
 import math
+import os
 from dataclasses import dataclass
 from typing import Optional, Union
 
@@ -27,41 +30,133 @@ class SchedulerOutput:
 
 
 class DDIMScheduler:
-    """Subset of diffusers' DDIMScheduler the reference touches: `set_timesteps`, `timesteps`,
-    `step(...).prev_sample / .pred_original_sample`, `alphas_cumprod`, `config`.  scaled-linear betas,
-    eta = 0, no clipping/thresholding (SD-2 config)."""
+    """diffusers' (0.30.2) DDIMScheduler as the reference uses it: `from_pretrained`, `set_timesteps` (trailing,
+    leading, linspace), `timesteps`, `step(...).prev_sample / .pred_original_sample`, `alphas_cumprod`,
+    `final_alpha_cumprod`, `config`.  Scaled-linear betas, eta = 0, no clipping / thresholding (the SD-2 and
+    Marigold / GeoWizard configs); `from_pretrained` rejects a config that needs anything else."""
+
+    # diffusers' constructor defaults: a key missing from scheduler_config.json takes these
+    _DIFFUSERS_DEFAULTS = dict(num_train_timesteps=1000, beta_start=0.0001, beta_end=0.02, beta_schedule="linear",
+                               trained_betas=None, clip_sample=True, set_alpha_to_one=True, steps_offset=0,
+                               prediction_type="epsilon", thresholding=False, dynamic_thresholding_ratio=0.995,
+                               clip_sample_range=1.0, sample_max_value=1.0, timestep_spacing="leading",
+                               rescale_betas_zero_snr=False)
+    _SPACINGS = ("trailing", "leading", "linspace")
 
     def __init__(self, num_train_timesteps=1000, beta_start=0.00085, beta_end=0.012,
-                 prediction_type="v_prediction", timestep_spacing="trailing", steps_offset=1):
+                 prediction_type="v_prediction", timestep_spacing="trailing", steps_offset=1, set_alpha_to_one=True):
         betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, num_train_timesteps, dtype=torch.float32) ** 2
         self.alphas_cumprod = torch.cumprod(1.0 - betas, dim=0)
-        self.final_alpha_cumprod = torch.tensor(1.0)
-        self.config = dict(num_train_timesteps=num_train_timesteps, prediction_type=prediction_type,
-                           timestep_spacing=timestep_spacing, steps_offset=steps_offset)
+        # the alpha of the step after the last one (diffusers: 1 with set_alpha_to_one, else alphas_cumprod[0])
+        self.final_alpha_cumprod = torch.tensor(1.0) if set_alpha_to_one else self.alphas_cumprod[0]
+        self.config = dict(num_train_timesteps=num_train_timesteps, beta_start=beta_start, beta_end=beta_end,
+                           beta_schedule="scaled_linear", prediction_type=prediction_type,
+                           timestep_spacing=timestep_spacing, steps_offset=steps_offset,
+                           set_alpha_to_one=set_alpha_to_one)
         self.num_inference_steps = None
         self.timesteps = None
         self._ac = [float(a) for a in self.alphas_cumprod]       # host copy: no device sync in step()
+        self._final_ac = float(self.final_alpha_cumprod)
+
+    @classmethod
+    def from_pretrained(cls, pretrained_model_name_or_path, subfolder=None, **kwargs):
+        """Read a diffusers `scheduler_config.json` (e.g. `from_pretrained(ckpt, subfolder="scheduler",
+        timestep_spacing="trailing")`, Marigold/run.py:273, GeoWizard/run_infer.py:194-197).  Keyword arguments
+        override the file.  A config whose math the engine does not implement raises ValueError naming the key."""
+        d = pretrained_model_name_or_path if subfolder is None else os.path.join(pretrained_model_name_or_path, subfolder)
+        with open(os.path.join(d, "scheduler_config.json")) as f:
+            cfg = json.load(f)
+        cfg.update(kwargs)
+        return cls.from_config(cfg)
+
+    @classmethod
+    def from_config(cls, config):
+        """Keys that are not DDIMScheduler arguments change no DDIM math and are kept, as diffusers ignores them (e.g.
+        `skip_prk_steps` of the SD-2 scheduler configs, a PNDM key): they land in `config["_extra"]`."""
+        cfg = dict(cls._DIFFUSERS_DEFAULTS)
+        cfg.update({k: v for k, v in config.items() if k in cls._DIFFUSERS_DEFAULTS})
+        extra = {k: v for k, v in config.items() if k not in cls._DIFFUSERS_DEFAULTS and k != "_class_name"}
+        if cfg["beta_schedule"] != "scaled_linear":
+            raise ValueError(f"beta_schedule={cfg['beta_schedule']!r}: the engine implements 'scaled_linear' only")
+        if cfg["trained_betas"] is not None:
+            raise ValueError("trained_betas: the engine implements the 'scaled_linear' schedule only")
+        for k in ("clip_sample", "thresholding", "rescale_betas_zero_snr"):
+            if cfg[k]:
+                raise ValueError(f"{k}=True is not supported by the engine (DDIM with eta = 0 and no clipping only)")
+        if cfg["prediction_type"] not in ops.PREDICTION_TYPES:
+            raise ValueError(f"prediction_type={cfg['prediction_type']!r} is not one of {sorted(ops.PREDICTION_TYPES)}")
+        if cfg["timestep_spacing"] not in cls._SPACINGS:
+            raise ValueError(f"timestep_spacing={cfg['timestep_spacing']!r} is not one of {list(cls._SPACINGS)}")
+        sched = cls(num_train_timesteps=int(cfg["num_train_timesteps"]), beta_start=float(cfg["beta_start"]),
+                    beta_end=float(cfg["beta_end"]), prediction_type=cfg["prediction_type"],
+                    timestep_spacing=cfg["timestep_spacing"], steps_offset=int(cfg["steps_offset"]),
+                    set_alpha_to_one=bool(cfg["set_alpha_to_one"]))
+        if extra:
+            sched.config["_extra"] = extra
+        return sched
 
     def set_timesteps(self, num_inference_steps, device=None):
         T = self.config["num_train_timesteps"]
+        if not 1 <= num_inference_steps <= T:
+            raise ValueError(f"num_inference_steps={num_inference_steps} must be in [1, num_train_timesteps={T}]")
         self.num_inference_steps = num_inference_steps
         if self.config["timestep_spacing"] == "trailing":
             ts = np.round(np.arange(T, 0, -T / num_inference_steps)) - 1
         elif self.config["timestep_spacing"] == "leading":
             ts = (np.arange(0, num_inference_steps) * (T // num_inference_steps)).round()[::-1].copy()
             ts = ts + self.config["steps_offset"]
+        elif self.config["timestep_spacing"] == "linspace":
+            ts = np.linspace(0, T - 1, num_inference_steps).round()[::-1].copy()
         else:
             raise ValueError(self.config["timestep_spacing"])
         self._host_timesteps = [int(t) for t in ts]
         self.timesteps = torch.tensor(self._host_timesteps, dtype=torch.long, device=device)
 
+    def prev_timestep(self, timestep):
+        """diffusers' `t - T // num_inference_steps` (so e.g. 3-step trailing 999 -> 666 -> 332 steps 666 to 333)."""
+        return int(timestep) - self.config["num_train_timesteps"] // self.num_inference_steps
+
     def coefficients(self, t_index):
         """(t, t_prev, a_t, a_prev) for the i-th inference step, all host floats/ints."""
         t = self._host_timesteps[t_index]
-        prev = t - self.config["num_train_timesteps"] // self.num_inference_steps
+        prev = self.prev_timestep(t)
         a_t = self._ac[t]
-        a_prev = self._ac[prev] if prev >= 0 else 1.0
+        a_prev = self._ac[prev] if prev >= 0 else self._final_ac
         return t, prev, a_t, a_prev
+
+    def step(self, model_output, timestep, sample, eta=0.0, return_dict=True):
+        """One DDIM update on the `b200_ddim_step` kernel -> SchedulerOutput(prev_sample, pred_original_sample), both
+        fp32 (the engine keeps the DDIM state in fp32 whatever the model dtype).  `timestep` is an int or a 0-d tensor
+        (a device tensor costs one host sync)."""
+        if eta != 0.0:
+            raise NotImplementedError("DDIMScheduler.step: eta != 0 (stochastic DDIM) is not implemented")
+        if self.num_inference_steps is None:
+            raise ValueError("call set_timesteps before step")
+        t = int(timestep)
+        T = self.config["num_train_timesteps"]
+        if not 0 <= t < T:
+            raise ValueError(f"timestep {t} is outside [0, num_train_timesteps={T})")
+        prev = self.prev_timestep(t)
+        a_prev = self._ac[prev] if prev >= 0 else self._final_ac
+        x = sample if sample.dtype == torch.float32 else sample.float()           # dtype cast at the API boundary
+        prev_sample, x0 = ops.ddim_step(model_output, x, self._ac[t], a_prev, self.config["prediction_type"],
+                                        want_x0=True)
+        if not return_dict:
+            return prev_sample, x0
+        return SchedulerOutput(prev_sample, x0)
+
+
+def _x0_coefficients(prediction_type, a_t):
+    """x0 = c_x * x_t + c_m * model_out: the scheduler's pred_original_sample as a linear map (fused into
+    post_quant_conv on the last step)."""
+    sa, sb = math.sqrt(a_t), math.sqrt(1.0 - a_t)
+    if prediction_type == "v_prediction":
+        return sa, -sb
+    if prediction_type == "epsilon":
+        return 1.0 / sa, -sb / sa
+    if prediction_type == "sample":
+        return 0.0, 1.0
+    raise ValueError(prediction_type)
 
 
 # ------------------------------------------------------------------------------------ base
@@ -117,31 +212,33 @@ class PipelineBase:
             self.__dict__["_wk_params"], self.__dict__["_wk_mods"] = ps, mods
         return (_WEIGHTS_EPOCH[0], hash(tuple((p.data_ptr(), p._version) for p in ps)))
 
-    def _graphed(self, key, fn, x):
-        """Capture `fn(static_x)` once per (key, weights version) and replay it; returns a fresh tensor."""
+    def _graphed(self, key, fn, *xs):
+        """Capture `fn(*static_xs)` once per (key, weights version) and replay it; returns a fresh tensor.  Every input
+        (the image batch, and the initial latent when the call draws noise) is copied into its static buffer first."""
         graphs = self.__dict__.setdefault("_graphs", {})
         wkey = self._weights_key()
         ent = graphs.get(key)
         if ent is None or ent["wkey"] != wkey:
-            static_x = x.clone()
+            static_xs = [x.clone() for x in xs]
             cur = torch.cuda.current_stream()
             side = torch.cuda.Stream()
             side.wait_stream(cur)
             with torch.cuda.stream(side):
                 for _ in range(2):                         # warm-up: packs weights, sets func attributes
-                    fn(static_x)
+                    fn(*static_xs)
             cur.wait_stream(side)
             torch.cuda.synchronize()
             before = (ops.STATS.launches, dict(ops.STATS.flops), dict(ops.STATS.count))
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                out = fn(static_x)
+                out = fn(*static_xs)
             delta = dict(launches=ops.STATS.launches - before[0],
                          flops={k: ops.STATS.flops[k] - before[1][k] for k in before[1]},
                          count={k: ops.STATS.count[k] - before[2][k] for k in before[2]})
-            ent = dict(g=g, x=static_x, out=out, wkey=wkey, delta=delta)
+            ent = dict(g=g, xs=static_xs, out=out, wkey=wkey, delta=delta)
             graphs[key] = ent
-        ent["x"].copy_(x, non_blocking=True)
+        for s, x in zip(ent["xs"], xs):
+            s.copy_(x, non_blocking=True)
         ent["g"].replay()
         d = ent["delta"]
         ops.STATS.launches += d["launches"]
@@ -177,6 +274,46 @@ def pyramid_noise_like(x, discount=0.9, generator=None):
         r = random.random() * 2 + 2
         w, h = max(1, int(w / (r ** i))), max(1, int(h / (r ** i)))
         noise += u(torch.randn(b, c, w, h, device=x.device, dtype=x.dtype, generator=generator)) * discount ** i
+        if w == 1 or h == 1:
+            break
+    return noise / noise.std()
+
+
+NOISE_TYPES = ("gaussian", "pyramid", "zeros")
+
+
+def _check_noise(noise, num_inference_steps):
+    """Argument checks of the denoising loop, raised before anything is launched."""
+    if noise not in NOISE_TYPES:
+        raise ValueError(f"Unknown noise type: {noise}")
+    if int(num_inference_steps) < 1:
+        raise ValueError(f"num_inference_steps={num_inference_steps} must be >= 1")
+
+
+def _check_geowizard_noise(noise, num_inference_steps):
+    """GeoWizard's pyramid noise adds `[T,1,1,1]`-shaped timesteps / 1000 in place into a `[B,...]` map: with T > 1 the
+    reference raises, except when B == T, where it silently scales each sample of the batch by a different timestep.
+    Neither is a defined schedule, so the engine refuses pyramid noise with more than one step."""
+    _check_noise(noise, num_inference_steps)
+    if noise == "pyramid" and num_inference_steps > 1:
+        raise ValueError("GeoWizard's pyramid noise (geowizard_pipeline.py:33-43) scales the noise by timesteps / 1000 "
+                         f"with an in-place broadcast that is only defined for one step; with {num_inference_steps} "
+                         "steps the reference raises (or, when the batch size equals the step count, scales each sample "
+                         "by a different timestep). Use noise='gaussian' or 'zeros', or num_inference_steps=1")
+
+
+def geowizard_pyramid_noise_like(x, timesteps, discount=0.9):
+    """GeoWizard's own multi-resolution noise (geowizard_pipeline.py:33-43): the coarser maps are scaled by
+    timesteps / 1000, r is drawn from numpy in [1.5, 3) and the coarse draws come from torch's CPU generator.  Not
+    Marigold's `pyramid_noise_like`.  Host-pipeline code; only defined for one timestep (see _check_geowizard_noise)."""
+    b, c, w_ori, h_ori = x.shape
+    u = torch.nn.Upsample(size=(w_ori, h_ori), mode="bilinear")
+    noise = torch.randn_like(x)
+    scale = 1.5
+    for i in range(10):
+        r = np.random.random() * scale + scale
+        w, h = max(1, int(w_ori / (r ** i))), max(1, int(h_ori / (r ** i)))
+        noise += u(torch.randn(b, c, w, h).to(x)) * (timesteps[..., None, None, None] / 1000) * discount ** i
         if w == 1 or h == 1:
             break
     return noise / noise.std()
@@ -223,6 +360,7 @@ class MarigoldPipeline(PipelineBase):
         assert processing_res >= 0 and ensemble_size >= 1
         if resample_method != "bilinear":
             raise NotImplementedError("the engine resizes with the reference's default (bilinear, antialiased)")
+        _check_noise(noise, denoising_steps)
         if isinstance(input_image, torch.Tensor):
             rgb = input_image.squeeze()
         else:                                              # PIL.Image
@@ -296,65 +434,84 @@ class MarigoldPipeline(PipelineBase):
             return torch.cat([self.single_infer(rgb_in[i:i + max_b], num_inference_steps, show_pbar, noise=noise,
                                                 normals=normals, generator=generator)
                               for i in range(0, B, max_b)], dim=0)
-        if (self.use_cuda_graph and noise == "zeros" and num_inference_steps == 1 and rgb_in.is_cuda
-                and not torch.cuda.is_current_stream_capturing()):
-            key = ("marigold", tuple(rgb_in.shape), rgb_in.dtype, bool(normals),
-                   bool(getattr(self.vae, "memory_efficient_attention", False)))
+        _check_noise(noise, num_inference_steps)
+        graph = self.use_cuda_graph and rgb_in.is_cuda and not torch.cuda.is_current_stream_capturing()
+        mem_eff = bool(getattr(self.vae, "memory_efficient_attention", False))
+        if graph and noise == "zeros" and num_inference_steps == 1:
+            key = ("marigold", tuple(rgb_in.shape), rgb_in.dtype, bool(normals), mem_eff)
             return self._graphed(key, lambda x: self._single_infer_impl(x, 1, noise, normals, None), rgb_in)
-        return self._single_infer_impl(rgb_in, num_inference_steps, noise, normals, generator)
+        # the initial latent is drawn here, outside any graph, on every call (marigold_pipeline.py:410-423)
+        init = None if noise == "zeros" else self._initial_latent(rgb_in, noise, generator)
+        if graph:
+            self.scheduler.set_timesteps(num_inference_steps)
+            sched = self.scheduler
+            key = ("marigold-ddim", tuple(rgb_in.shape), rgb_in.dtype, bool(normals), mem_eff,
+                   tuple(sched._host_timesteps), sched.config["prediction_type"], sched._final_ac, init is None,
+                   tuple(sched.coefficients(i) for i in range(num_inference_steps)))
+            if init is None:
+                return self._graphed(key, lambda x: self._single_infer_impl(x, num_inference_steps, noise, normals,
+                                                                            None), rgb_in)
+            return self._graphed(key, lambda x, z: self._single_infer_impl(x, num_inference_steps, noise, normals,
+                                                                           None, init_latent=z), rgb_in, init)
+        return self._single_infer_impl(rgb_in, num_inference_steps, noise, normals, generator, init_latent=init)
 
-    def _single_infer_impl(self, rgb_in, num_inference_steps, noise, normals, generator):
+    def _latent_shape(self, rgb_in):
+        """[B, latent_channels, h, w] of encode_rgb(rgb_in): every VAE down-sampling conv (pad (0,1,0,1), stride 2)
+        floors the size."""
+        B, _, h, w = rgb_in.shape
+        for _ in range(len(self.vae.config["block_out_channels"]) - 1):
+            h, w = h // 2, w // 2
+        return B, self.vae.config["latent_channels"], h, w
+
+    def _initial_latent(self, rgb_in, noise, generator):
+        """The reference's initial latent (marigold_pipeline.py:410-423), in the module dtype; host-pipeline code."""
+        shape = self._latent_shape(rgb_in)
+        if noise == "gaussian":
+            return torch.randn(shape, device=rgb_in.device, dtype=self.dtype, generator=generator)
+        return pyramid_noise_like(torch.empty(shape, device=rgb_in.device, dtype=self.dtype), generator=generator)
+
+    def _single_infer_impl(self, rgb_in, num_inference_steps, noise, normals, generator, init_latent=None):
         device = rgb_in.device
         self.scheduler.set_timesteps(num_inference_steps)        # host-side only: graph-capture safe
         rgb_latent = self.encode_rgb(rgb_in)
-        if noise == "gaussian":
-            latent = torch.randn(rgb_latent.shape, device=device, dtype=rgb_latent.dtype, generator=generator)
-        elif noise == "pyramid":
-            latent = pyramid_noise_like(rgb_latent, generator=generator)
-        elif noise == "zeros":
-            latent = None                                   # exact zeros: never materialised
-        else:
-            raise ValueError(f"Unknown noise type: {noise}")
+        if noise != "zeros" and init_latent is None:
+            init_latent = self._initial_latent(rgb_in, noise, generator)
         if self.empty_text_embed is None:
             self.encode_empty_text()
         # one context for the whole batch (marigold_pipeline.py:428-432 `.repeat`s it): passed as a broadcast view so
         # the UNet can take its constant-context cross-attention path (same values, no copy)
         ctx = self.empty_text_embed.to(device).expand(rgb_latent.shape[0], -1, -1)
-        zeros = None
         spec = getattr(self.unet, "single_step_specialisations", False)
         pt = self.scheduler.config["prediction_type"]
+        # DDIM state x_t in fp32 whatever the module dtype; None = exact zeros (never materialised)
+        latent = None if init_latent is None else init_latent.to(torch.float32, memory_format=torch.contiguous_format,
+                                                                  copy=True)
+        unet_in = None
+        if latent is not None or not spec or num_inference_steps > 1:
+            # one persistent [B, 8, h, w] UNet input: [rgb_latent | x_t] (this order is important, :447-449); every
+            # intermediate DDIM step writes x_{t-1} into channels 4..7 in the UNet operand dtype
+            B, c, h, w = rgb_latent.shape
+            unet_in = torch.empty((B, 2 * c, h, w), dtype=rgb_latent.dtype, device=device)
+            unet_in[:, :c].copy_(rgb_latent)
+            if init_latent is None:
+                unet_in[:, c:].zero_()
+            else:
+                unet_in[:, c:].copy_(init_latent)
         for i in range(num_inference_steps):
             t, _, a_t, a_prev = self.scheduler.coefficients(i)
             if latent is None and spec:
-                cur = None
                 unet_input = rgb_latent                               # the zero half is never materialised: conv_in on 4 channels
             else:
-                if latent is None:
-                    zeros = torch.zeros_like(rgb_latent) if zeros is None else zeros
-                    cur = zeros
-                else:
-                    cur = latent
-                unet_input = torch.cat([rgb_latent, cur], dim=1)      # this order is important (:447-449)
+                unet_input = unet_in
             pred = self.unet(unet_input, t, encoder_hidden_states=ctx).sample
-            sa, sb = math.sqrt(a_t), math.sqrt(1.0 - a_t)
-            # x0 = c_x * x_t + c_m * model_out  (DDIM, eta = 0)
-            if pt == "v_prediction":
-                c_x, c_m = sa, -sb
-            elif pt == "epsilon":
-                c_x, c_m = 1.0 / sa, -sb / sa
-            elif pt == "sample":
-                c_x, c_m = 0.0, 1.0
-            else:
-                raise ValueError(pt)
             if i == num_inference_steps - 1:
-                # last step: latent = pred_original_sample, fused with /scale + post_quant_conv + decoder
+                # last step: latent = pred_original_sample, x0 = c_x * x_t + c_m * model_out fused with /scale +
+                # post_quant_conv + decoder
+                c_x, c_m = _x0_coefficients(pt, a_t)
                 dec = self.vae.decode_from_prediction(pred, c_m, noisy=latent, c_noisy=c_x)
                 break
-            # intermediate DDIM step (eta = 0): x_prev = sqrt(a_prev) x0 + sqrt(1-a_prev) eps
-            x_t = cur if cur is not None else torch.zeros_like(rgb_latent)
-            x0 = c_x * x_t + c_m * pred
-            eps = (x_t - sa * x0) / sb
-            latent = math.sqrt(a_prev) * x0 + math.sqrt(1.0 - a_prev) * eps
+            # intermediate DDIM step (eta = 0), one kernel: x_t -> x_{t-1} in place and into the next UNet input
+            latent, _ = ops.ddim_step(pred, latent, a_t, a_prev, pt, out=latent, unet_in=unet_in[:, rgb_latent.shape[1]:])
         if normals:
             return ops.decode_post(dec.float().contiguous(), normals=True).to(dec.dtype)
         return ops.decode_post(dec.float().contiguous(), normals=False).to(dec.dtype)
@@ -404,15 +561,22 @@ class DepthNormalEstimationPipeline(PipelineBase):
 
     @torch.no_grad()
     def single_infer(self, input_rgb, num_inference_steps: int, domain: str, show_pbar: bool = False,
-                     noise="zeros", img_embed=None):
+                     noise="zeros", img_embed=None, generator=None):
+        """geowizard_pipeline.py:251-344: any number of DDIM steps on the joint [depth x B, normal x B] latent, from
+        zeros, gaussian (one draw shared by both halves, :271-272) or GeoWizard's pyramid noise (:33-43)."""
+        _check_geowizard_noise(noise, num_inference_steps)
         device = input_rgb.device
         B = input_rgb.shape[0]
         _check_image_size(input_rgb.shape[-2], input_rgb.shape[-1])
         self.scheduler.set_timesteps(num_inference_steps, device=device)
-        if num_inference_steps != 1 or noise != "zeros":
-            raise NotImplementedError("engine pipeline implements the E2E-FT setting: 1 step, zeros noise")
         rgb_latent = self.encode_RGB(input_rgb)
-        geo_latent = torch.zeros_like(rgb_latent).repeat(2, 1, 1, 1)
+        if noise == "gaussian":
+            geo_init = torch.randn(rgb_latent.shape, device=device, dtype=self.dtype,
+                                   generator=generator).repeat(2, 1, 1, 1)
+        elif noise == "pyramid":
+            geo_init = geowizard_pyramid_noise_like(rgb_latent, self.scheduler.timesteps).repeat(2, 1, 1, 1)
+        else:
+            geo_init = None
         rgb_latent = rgb_latent.repeat(2, 1, 1, 1)
         emb = img_embed if img_embed is not None else self.img_embed
         if emb is None and self.image_encoder is not None:
@@ -422,16 +586,51 @@ class DepthNormalEstimationPipeline(PipelineBase):
         ctx = emb.to(device)
         ctx = ctx.repeat(2, 1, 1) if ctx.shape[0] == B else ctx.repeat(2 * B, 1, 1)
         cls = self.class_embedding(domain, B, device, rgb_latent.dtype)
-        t, _, a_t, _ = self.scheduler.coefficients(0)
-        pred = self.unet(torch.cat([rgb_latent, geo_latent], dim=1), torch.full((2 * B,), t, device=device),
-                         encoder_hidden_states=ctx, class_labels=cls).sample
-        assert self.scheduler.config["prediction_type"] == "v_prediction"
-        c_m = -math.sqrt(1.0 - a_t)
-        d = self.vae.decode_from_prediction(pred[:B].contiguous(), c_m)
-        n = self.vae.decode_from_prediction(pred[B:].contiguous(), c_m)
+        if num_inference_steps == 1 and geo_init is None:
+            # the E2E-FT setting (1 step, zeros): x_t = 0, so x0 = c_m * model_out
+            geo_latent = torch.zeros_like(rgb_latent)
+            t, _, a_t, _ = self.scheduler.coefficients(0)
+            pred = self.unet(torch.cat([rgb_latent, geo_latent], dim=1), torch.full((2 * B,), t, device=device),
+                             encoder_hidden_states=ctx, class_labels=cls).sample
+            assert self.scheduler.config["prediction_type"] == "v_prediction"
+            c_m = -math.sqrt(1.0 - a_t)
+            d = self.vae.decode_from_prediction(pred[:B].contiguous(), c_m)
+            n = self.vae.decode_from_prediction(pred[B:].contiguous(), c_m)
+        else:
+            d, n = self._denoise(rgb_latent, geo_init, num_inference_steps, ctx, cls)
         depth = ops.decode_post(d.float().contiguous(), normals=False).to(d.dtype)
         normal = ops.decode_post(n.float().contiguous(), normals=True, sign=-1.0).to(n.dtype)   # :342 sign flip
         return depth, normal
+
+    def _denoise(self, rgb_latent, geo_init, num_inference_steps, ctx, cls):
+        """The DDIM loop of :319-334 on the [2B] state (eager): unet(.., t.repeat(2B), class_labels) then one
+        `ddim_step` kernel per intermediate step; the last step's x0 is fused into post_quant_conv for both halves.
+        Returns the decoded (depth, normal) halves."""
+        device = rgb_latent.device
+        B2, c = rgb_latent.shape[:2]
+        B = B2 // 2
+        pt = self.scheduler.config["prediction_type"]
+        latent = None if geo_init is None else geo_init.to(torch.float32, memory_format=torch.contiguous_format,
+                                                             copy=True)
+        unet_in = torch.empty((B2, 2 * c) + tuple(rgb_latent.shape[2:]), dtype=rgb_latent.dtype, device=device)
+        unet_in[:, :c].copy_(rgb_latent)
+        if geo_init is None:
+            unet_in[:, c:].zero_()
+        else:
+            unet_in[:, c:].copy_(geo_init)
+        for i in range(num_inference_steps):
+            t, _, a_t, a_prev = self.scheduler.coefficients(i)
+            pred = self.unet(unet_in, torch.full((B2,), t, device=device), encoder_hidden_states=ctx,
+                             class_labels=cls).sample
+            if i == num_inference_steps - 1:
+                c_x, c_m = _x0_coefficients(pt, a_t)
+                halves = []
+                for sl in (slice(0, B), slice(B, B2)):
+                    noisy = None if latent is None else latent[sl]
+                    halves.append(self.vae.decode_from_prediction(pred[sl].contiguous(), c_m, noisy=noisy,
+                                                                  c_noisy=c_x))
+                return halves[0], halves[1]
+            latent, _ = ops.ddim_step(pred, latent, a_t, a_prev, pt, out=latent, unet_in=unet_in[:, c:])
 
     @torch.no_grad()
     def encode_img_embed(self, rgb):
@@ -458,7 +657,10 @@ class DepthNormalEstimationPipeline(PipelineBase):
     @torch.no_grad()
     def __call__(self, input_image, denoising_steps: int = 1, ensemble_size: int = 1, processing_res: int = 768,
                  match_input_res: bool = True, domain: str = "indoor", color_map: Optional[str] = None,
-                 show_progress_bar: bool = False, noise="zeros", img_embed=None) -> DepthNormalPipelineOutput:
+                 show_progress_bar: bool = False, noise="zeros", img_embed=None,
+                 batch_size: int = 0) -> DepthNormalPipelineOutput:
+        _check_geowizard_noise(noise, denoising_steps)
+        assert ensemble_size >= 1 and batch_size >= 0
         if isinstance(input_image, torch.Tensor):
             rgb = input_image.squeeze()
         else:
@@ -471,8 +673,10 @@ class DepthNormalEstimationPipeline(PipelineBase):
             rgb = _resize_max_res(rgb, processing_res)
         rgb_norm = normalise_rgb(rgb, round_u8=was_u8 and processing_res > 0).to(self.dtype)
         dl, nl = [], []
-        for _ in range(ensemble_size):                      # geowizard_pipeline.py:139-176 (batch size 1 per member)
-            d, n = self.single_infer(rgb_norm[None], denoising_steps, domain, show_progress_bar, noise, img_embed)
+        bs = batch_size if batch_size > 0 else 1            # geowizard_pipeline.py:139-176 (0 -> one member per batch)
+        for i in range(0, ensemble_size, bs):
+            batch = rgb_norm[None].expand(min(bs, ensemble_size - i), -1, -1, -1).contiguous()
+            d, n = self.single_infer(batch, denoising_steps, domain, show_progress_bar, noise, img_embed)
             dl.append(d)
             nl.append(n)
         depth, normal = torch.cat(dl).squeeze(), torch.cat(nl).squeeze()

@@ -186,6 +186,27 @@ int b200_pointwise_nchw(const float* in1, float a1, const float* in2, float a2, 
                         const float* Wm, const float* bias, int NB, int Cin, int Cout, long long HW,
                         float* out, void* stream);
 
+/* One DDIM update (diffusers DDIMScheduler.step, eta = 0) on NCHW latents, fp32 arithmetic in diffusers' order:
+ *   beta = 1 - a_t;  x0, eps from the prediction type:
+ *     B200_PRED_V:       x0 = sqrt(a_t) x - sqrt(beta) m,   eps = sqrt(a_t) m + sqrt(beta) x
+ *     B200_PRED_EPSILON: x0 = (x - sqrt(beta) m) / sqrt(a_t), eps = m
+ *     B200_PRED_SAMPLE:  x0 = m,                            eps = (x - sqrt(a_t) x0) / sqrt(beta)
+ *   prev = sqrt(a_prev) x0 + sqrt(1 - a_prev) eps.
+ * model_out m: [B][C][HW] (mo_f16 ? fp16 : fp32), batch stride mo_bstride; sample x: fp32, batch stride s_bstride,
+ * NULL = exact zeros.  prev_sample: fp32 [B][C][HW] contiguous, may alias sample (then s_bstride = C*HW);
+ * pred_original_sample: fp32 [B][C][HW] or NULL.  unet_in (nullable): prev cast to fp16 (unet_in_f16) or fp32, written
+ * at unet_in[b*ui_bstride + c*HW + p] -- the noisy-latent channel slice of the next step's UNet input, so the
+ * per-step concatenation and cast disappear.  0 < a_t < 1, 0 <= a_prev <= 1.
+ * Replaces scheduler.step at Marigold/marigold/marigold_pipeline.py:457-465 and
+ * GeoWizard/geowizard/models/geowizard_pipeline.py:326-334. */
+#define B200_PRED_EPSILON 0
+#define B200_PRED_V 1
+#define B200_PRED_SAMPLE 2
+int b200_ddim_step(const void* model_out, int mo_f16, long long mo_bstride, const float* sample, long long s_bstride,
+                   int B, int C, long long HW, int prediction_type, float alpha_prod_t, float alpha_prod_t_prev,
+                   float* prev_sample, float* pred_original_sample, void* unet_in, int unet_in_f16,
+                   long long ui_bstride, void* stream);
+
 /* Decode post-ops on NCHW fp32 [B][3][HW]: mode 0 = depth: (clip(mean_c, -1, 1)+1)/2 -> [B][1][HW];
  * mode 1 = normals: x/(||x||_2+1e-5) * sign -> [B][3][HW] (marigold_pipeline.py:467-478);
  * mode 2 / 3 = the training variants: clip(mean_c) without the affine map / normalised then clamped
