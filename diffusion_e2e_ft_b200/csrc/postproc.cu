@@ -302,6 +302,100 @@ __global__ void resize_nearest_kernel(const float* __restrict__ x, long long pla
   }
 }
 
+// torch's `nearest-exact` resize of a [planes][H][W] fp32 tensor (the reference's resample_method="nearest",
+// Marigold/marigold/util/image_util.py:115 NEAREST_EXACT): src = min(floor((dst + 0.5) * scale), in - 1) with the fp32
+// scale in / out of aten's CUDA kernel (compute_scales_value), each operation rounded on its own.
+// blockIdx.y strides over the planes * OH output rows (the source row is resolved once per row), x over the columns.
+__global__ void resize_nearest_exact_kernel(const float* __restrict__ x, long long rows, int H, int W, int OH, int OW,
+                                            float sh, float sw, float* __restrict__ out) {
+  for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
+    const int oh = (int)(r % OH);
+    const long long pl = r / OH;
+    const int ih = min((int)floorf(__fmul_rn(__fadd_rn((float)oh, 0.5f), sh)), H - 1);
+    const float* __restrict__ src = x + (pl * H + ih) * W;
+    float* __restrict__ dst = out + r * OW;
+    for (int ow = blockIdx.x * blockDim.x + threadIdx.x; ow < OW; ow += gridDim.x * blockDim.x) {
+      const int iw = min((int)floorf(__fmul_rn(__fadd_rn((float)ow, 0.5f), sw)), W - 1);
+      dst[ow] = src[iw];
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------ colouring
+// Both colour kernels write uint8 HWC.  A thread owns a group of 4 pixels, so its 12 output bytes go out as three
+// aligned 32-bit stores (the output base is 4-byte aligned); the n % 4 tail is written byte by byte.
+__device__ __forceinline__ void store_rgb4(unsigned char* __restrict__ out, long long g, const unsigned char (&c)[12]) {
+  unsigned int* o = reinterpret_cast<unsigned int*>(out + 12 * g);
+#pragma unroll
+  for (int w = 0; w < 3; ++w)
+    o[w] = (unsigned)c[4 * w] | ((unsigned)c[4 * w + 1] << 8) | ((unsigned)c[4 * w + 2] << 16) |
+           ((unsigned)c[4 * w + 3] << 24);
+}
+
+// matplotlib Colormap.__call__(clip(x, 0, 1)) on a float32 array: xa = x * N (one fp32 multiply), xa == N -> N - 1,
+// int truncation, NaN -> the "bad" colour (0, 0, 0).  table [n][3] uint8 already holds (lut * 255).astype(uint8).
+__device__ __forceinline__ int cmap_index(float v, int n, float fn) {
+  v = fminf(fmaxf(v, 0.f), 1.f);
+  const int k = (int)__fmul_rn(v, fn);
+  return k >= n ? n - 1 : k;
+}
+
+__global__ void colorize_depth_kernel(const float* __restrict__ x, long long n, const unsigned char* __restrict__ table,
+                                      int ncol, unsigned char* __restrict__ out) {
+  extern __shared__ unsigned char s_tab[];
+  for (int i = threadIdx.x; i < 3 * ncol; i += blockDim.x) s_tab[i] = table[i];
+  __syncthreads();
+  const float fn = (float)ncol;
+  const long long groups = n / 4;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    unsigned char c[12];
+#pragma unroll
+    for (int p = 0; p < 4; ++p) {
+      const float v = x[4 * g + p];
+      const int k = cmap_index(v, ncol, fn);
+      const bool bad = isnan(v);
+      c[3 * p] = bad ? 0 : s_tab[3 * k];
+      c[3 * p + 1] = bad ? 0 : s_tab[3 * k + 1];
+      c[3 * p + 2] = bad ? 0 : s_tab[3 * k + 2];
+    }
+    store_rgb4(out, g, c);
+  }
+  for (long long i = 4 * groups + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float v = x[i];
+    const int k = cmap_index(v, ncol, fn);
+    const bool bad = isnan(v);
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) out[3 * i + ch] = bad ? 0 : s_tab[3 * k + ch];
+  }
+}
+
+// numpy's ((clip(x, -1, 1) + 1) / 2 * 255).astype(uint8) on float32 (marigold_pipeline.py:340-343,
+// geowizard_pipeline.py:219): every operation rounded separately (no FMA contraction), truncated; NaN -> 0.
+__device__ __forceinline__ unsigned char normal_u8(float v) {
+  if (isnan(v)) return 0;
+  v = fminf(fmaxf(v, -1.f), 1.f);
+  return (unsigned char)__float2uint_rz(__fmul_rn(__fdiv_rn(__fadd_rn(v, 1.f), 2.f), 255.f));
+}
+
+// x [3][HW] planar -> out [HW][3]
+__global__ void colorize_normals_kernel(const float* __restrict__ x, long long HW, unsigned char* __restrict__ out) {
+  const long long groups = HW / 4;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += stride) {
+    unsigned char c[12];
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) c[3 * p + ch] = normal_u8(x[ch * HW + 4 * g + p]);
+    store_rgb4(out, g, c);
+  }
+  for (long long i = 4 * groups + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += stride) {
+#pragma unroll
+    for (int ch = 0; ch < 3; ++ch) out[3 * i + ch] = normal_u8(x[ch * HW + i]);
+  }
+}
+
 static unsigned pp_grid(long long n, int per_thread = 4) {
   long long g = (n + 256LL * per_thread - 1) / (256LL * per_thread);
   const long long cap = (long long)sm_count() * 8;
@@ -421,5 +515,33 @@ extern "C" int b200_resize_nearest(const float* x, long long planes, int H, int 
   B200_CHECK_ARG(x && out && planes > 0 && H > 0 && W > 0 && OH > 0 && OW > 0, "b200_resize_nearest: bad arguments");
   resize_nearest_kernel<<<pp_grid(planes * OH * OW, 1), 256, 0, (cudaStream_t)stream>>>(x, planes, H, W, OH, OW, out);
   B200_CHECK_LAUNCH("resize_nearest_kernel");
+  return 0;
+}
+
+extern "C" int b200_resize_nearest_exact(const float* x, long long planes, int H, int W, int OH, int OW, float* out,
+                                         void* stream) {
+  B200_CHECK_ARG(x && out && planes > 0 && H > 0 && W > 0 && OH > 0 && OW > 0, "b200_resize_nearest_exact: bad arguments");
+  const float sh = (float)H / (float)OH, sw = (float)W / (float)OW;
+  const long long rows = planes * OH;
+  const dim3 grid((unsigned)((OW + 255) / 256), (unsigned)(rows < 65535 ? rows : 65535));
+  resize_nearest_exact_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, rows, H, W, OH, OW, sh, sw, out);
+  B200_CHECK_LAUNCH("resize_nearest_exact_kernel");
+  return 0;
+}
+
+extern "C" int b200_colorize_depth(const float* x, long long n, const unsigned char* table, int ncol,
+                                   unsigned char* out, void* stream) {
+  B200_CHECK_ARG(x && table && out && n > 0 && ncol > 0 && ncol <= 4096, "b200_colorize_depth: bad arguments");
+  B200_CHECK_ARG(((uintptr_t)out & 3) == 0, "b200_colorize_depth: out must be 4-byte aligned");
+  colorize_depth_kernel<<<pp_grid(n), 256, 3 * ncol, (cudaStream_t)stream>>>(x, n, table, ncol, out);
+  B200_CHECK_LAUNCH("colorize_depth_kernel");
+  return 0;
+}
+
+extern "C" int b200_colorize_normals(const float* x, long long HW, unsigned char* out, void* stream) {
+  B200_CHECK_ARG(x && out && HW > 0, "b200_colorize_normals: bad arguments");
+  B200_CHECK_ARG(((uintptr_t)out & 3) == 0, "b200_colorize_normals: out must be 4-byte aligned");
+  colorize_normals_kernel<<<pp_grid(HW), 256, 0, (cudaStream_t)stream>>>(x, HW, out);
+  B200_CHECK_LAUNCH("colorize_normals_kernel");
   return 0;
 }

@@ -3,6 +3,8 @@
     ensemble_normals   <- Marigold/marigold/marigold_pipeline.py:59-71 == GeoWizard/geowizard/utils/normal_ensemble.py:6-22
     ensemble_depths    <- Marigold/marigold/util/ensemble.py:40-132
     resize_bilinear_aa / normalise_rgb / minmax_normalise <- marigold_pipeline.py:237-247,300-321
+    resize_bicubic_aa / resize_nearest_exact <- the other two resample_method choices (:219,237-242,315-321)
+    colorize_depth / colorize_normals <- marigold_pipeline.py:327-343, geowizard_pipeline.py:211-219
 
 Signatures, argument meaning and return values are the reference's.  The arithmetic runs in libb200_e2eft.so
 (csrc/postproc.cu); torch only allocates.  `ensemble_depths` keeps the reference's optimiser — scipy's BFGS driven
@@ -103,6 +105,103 @@ def resize_nearest(x: torch.Tensor, size):
     planes = xf.numel() // (H * W)
     out = torch.empty((*xf.shape[:-2], OH, OW), dtype=F32, device=x.device)
     _ck(_lib.load().b200_resize_nearest(_p(xf), planes, H, W, OH, OW, _p(out), _stream()), "b200_resize_nearest")
+    return out
+
+
+def resize_nearest_exact(x: torch.Tensor, size):
+    """torch `interpolate(x, size, mode="nearest-exact")` of a [..., H, W] CUDA tensor: the reference's
+    resample_method="nearest" (torchvision NEAREST_EXACT, Marigold/marigold/util/image_util.py:111-116)."""
+    _need_cuda(x)
+    xf = x.to(F32).contiguous()
+    H, W = xf.shape[-2:]
+    OH, OW = int(size[0]), int(size[1])
+    planes = xf.numel() // (H * W)
+    out = torch.empty((*xf.shape[:-2], OH, OW), dtype=F32, device=x.device)
+    _ck(_lib.load().b200_resize_nearest_exact(_p(xf), planes, H, W, OH, OW, _p(out), _stream()),
+        "b200_resize_nearest_exact")
+    return out
+
+
+# ------------------------------------------------------------------------------------ colour maps
+# matplotlib is not a dependency, so the one colour map the reference pipelines default to ("Spectral") is derived
+# here the way matplotlib builds and applies it, in numpy float64:
+#   * matplotlib/_cm.py `_Spectral_data`: the 11 ColorBrewer control colours, each component k / 255;
+#   * matplotlib/colors.py `LinearSegmentedColormap.from_list(name, colors, N=256)`: the colours sit at
+#     np.linspace(0, 1, 11), each channel a segment table [x, y0, y1] with y0 == y1;
+#   * `_create_lookup_table(N, data, gamma=1)`: x * (N - 1), searchsorted of (N - 1) * linspace(0, 1, N) over it for
+#     the interior entries, linear interpolation, the two end entries copied from the table ends, clipped to [0, 1];
+#   * `Colormap.__call__(X, bytes=False)` returns lut[index] as float64, and the reference pipelines store
+#     `(colored * 255).astype(np.uint8)` (Marigold/marigold/marigold_pipeline.py:331-336,
+#     GeoWizard/geowizard/models/geowizard_pipeline.py:211-216): that truncation is folded into the uint8 table, so
+#     the device kernel only clips, indexes and gathers.
+SPECTRAL_CONTROL_RGB = ((158, 1, 66), (213, 62, 79), (244, 109, 67), (253, 174, 97), (254, 224, 139), (255, 255, 191),
+                        (230, 245, 152), (171, 221, 164), (102, 194, 165), (50, 136, 189), (94, 79, 162))
+COLOR_MAPS = ("Spectral",)
+_LUT_SIZE = 256
+
+
+def _create_lookup_table(N, x, y0, y1):
+    """matplotlib.colors._create_lookup_table(N, np.column_stack([x, y0, y1]), gamma=1.0) for N > 1."""
+    x = x * (N - 1)
+    xind = (N - 1) * np.linspace(0, 1, N)
+    ind = np.searchsorted(x, xind)[1:-1]
+    distance = (xind[1:-1] - x[ind - 1]) / (x[ind] - x[ind - 1])
+    lut = np.concatenate([[y1[0]], distance * (y0[ind] - y1[ind - 1]) + y1[ind - 1], [y0[-1]]])
+    return np.clip(lut, 0.0, 1.0)
+
+
+def spectral_lut(N=_LUT_SIZE):
+    """matplotlib's "Spectral" lookup table: float64 [N, 3] in [0, 1]."""
+    rgb = np.array(SPECTRAL_CONTROL_RGB, dtype=np.float64) / 255
+    vals = np.linspace(0, 1, len(rgb))
+    return np.stack([_create_lookup_table(N, vals, rgb[:, c], rgb[:, c]) for c in range(3)], axis=1)
+
+
+def check_color_map(cmap):
+    """None (no depth colouring) or a built-in colour map name; anything else raises before any launch."""
+    if cmap is not None and cmap not in COLOR_MAPS:
+        raise ValueError(f"color_map={cmap!r}: only {' / '.join(repr(c) for c in COLOR_MAPS)} is built in "
+                         "(or None for no depth colouring)")
+
+
+_TABLES = {}
+
+
+def _color_table(cmap, device):
+    """The uint8 [N, 3] table of `cmap` (a name in COLOR_MAPS) on `device`, built once per device."""
+    key = (cmap, device)
+    t = _TABLES.get(key)
+    if t is None:
+        table = (spectral_lut() * 255).astype(np.uint8)
+        t = _TABLES[key] = torch.from_numpy(np.ascontiguousarray(table)).to(device)
+    return t
+
+
+def colorize_depth(x: torch.Tensor, cmap="Spectral"):
+    """[H, W] (or [1, H, W]) fp32 depth in [0, 1] -> uint8 [H, W, 3] CUDA tensor: the reference's
+    `colorize_depth_maps(pred, 0, 1, cmap)` -> `(colored * 255).astype(np.uint8)` -> `chw2hwc`
+    (marigold_pipeline.py:327-338).  Values are clipped to [0, 1]; NaN gives (0, 0, 0)."""
+    check_color_map(cmap)
+    _need_cuda(x)
+    xf = x.to(F32).contiguous()
+    H, W = xf.shape[-2:]
+    assert xf.numel() == H * W, f"colorize_depth takes one [H, W] map, got {tuple(x.shape)}"
+    table = _color_table(cmap, xf.device)
+    out = torch.empty((H, W, 3), dtype=torch.uint8, device=xf.device)
+    _ck(_lib.load().b200_colorize_depth(_p(xf), H * W, _p(table), table.shape[0], _p(out), _stream()),
+        "b200_colorize_depth")
+    return out
+
+
+def colorize_normals(x: torch.Tensor):
+    """[3, H, W] fp32 normals -> uint8 [H, W, 3] CUDA tensor: ((clip(x, -1, 1) + 1) / 2 * 255).astype(np.uint8) in
+    HWC (marigold_pipeline.py:339-343, geowizard_pipeline.py:218-219).  NaN gives 0."""
+    _need_cuda(x)
+    xf = x.to(F32).contiguous()
+    assert xf.dim() == 3 and xf.shape[0] == 3, f"colorize_normals takes [3, H, W], got {tuple(x.shape)}"
+    H, W = xf.shape[-2:]
+    out = torch.empty((H, W, 3), dtype=torch.uint8, device=xf.device)
+    _ck(_lib.load().b200_colorize_normals(_p(xf), H * W, _p(out), _stream()), "b200_colorize_normals")
     return out
 
 

@@ -257,8 +257,9 @@ class MarigoldDepthOutput:
     normal_colored: Optional[object]
 
 
-from .ensemble import (ensemble_depths, ensemble_normals, minmax_normalise_, minmax_rows, normalise_rgb,  # noqa: E402
-                       resize_bilinear_aa, resize_nearest)
+from .ensemble import (check_color_map, colorize_depth, colorize_normals, ensemble_depths,  # noqa: E402
+                       ensemble_normals, minmax_normalise_, minmax_rows, normalise_rgb, resize_bicubic_aa,
+                       resize_bilinear_aa, resize_nearest, resize_nearest_exact)
 
 
 def pyramid_noise_like(x, discount=0.9, generator=None):
@@ -336,11 +337,36 @@ def _max_res_size(h, w, max_edge):
     return int(h * s), int(w * s)
 
 
-def _resize_max_res(img, max_edge):
-    """Marigold/marigold/util/image_util.py:79-108 resize_max_res: antialiased bilinear down-scale to a maximum edge
-    length, on the device (csrc/postproc.cu)."""
+RESAMPLE_METHODS = ("bilinear", "bicubic", "nearest")
+
+
+def _check_resample_method(method):
+    """Marigold/marigold/util/image_util.py:111-120 get_tv_resample_method, raised before anything is launched."""
+    if method not in RESAMPLE_METHODS:
+        raise ValueError(f"Unknown resampling method: {method!r} (one of {list(RESAMPLE_METHODS)})")
+
+
+def _resize(x, size, method):
+    """torchvision `resize(x, size, method, antialias=True)` of a [..., H, W] fp32 tensor on the device:
+    "bilinear" / "bicubic" antialiased, "nearest" = NEAREST_EXACT (antialias does not apply)."""
+    if method == "bilinear":
+        return resize_bilinear_aa(x, size)
+    if method == "bicubic":
+        return resize_bicubic_aa(x, size)
+    return resize_nearest_exact(x, size)
+
+
+def _resize_max_res(img, max_edge, method="bilinear"):
+    """Marigold/marigold/util/image_util.py:79-108 resize_max_res: down-scale to a maximum edge length with the
+    chosen resampling (antialiased bilinear by default), on the device (csrc/postproc.cu)."""
     _, h, w = img.shape
-    return resize_bilinear_aa(img, _max_res_size(h, w, max_edge))
+    return _resize(img, _max_res_size(h, w, max_edge), method)
+
+
+def _to_pil(u8_hwc):
+    """uint8 [H, W, 3] device tensor -> PIL image (one device-to-host copy)."""
+    from PIL import Image
+    return Image.fromarray(u8_hwc.cpu().numpy())
 
 
 class MarigoldPipeline(PipelineBase):
@@ -358,8 +384,8 @@ class MarigoldPipeline(PipelineBase):
                  batch_size: int = 0, color_map: Optional[str] = "Spectral", show_progress_bar: bool = True,
                  ensemble_kwargs=None, noise="gaussian", normals=False) -> MarigoldDepthOutput:
         assert processing_res >= 0 and ensemble_size >= 1
-        if resample_method != "bilinear":
-            raise NotImplementedError("the engine resizes with the reference's default (bilinear, antialiased)")
+        _check_resample_method(resample_method)
+        check_color_map(color_map)
         _check_noise(noise, denoising_steps)
         if isinstance(input_image, torch.Tensor):
             rgb = input_image.squeeze()
@@ -369,12 +395,13 @@ class MarigoldPipeline(PipelineBase):
         assert rgb.dim() == 3 and input_size[0] == 3, f"Wrong input shape {input_size}, expected [rgb, H, W]"
         _check_image_size(*_max_res_size(input_size[-2], input_size[-1], processing_res))   # before any launch
         # pre-processing on the device (SURVEY.md §8 f2): the raw (uint8) image is uploaded once; resize + [0,255] ->
-        # [-1,1] run as kernels (marigold_pipeline.py:237-247)
+        # [-1,1] run as kernels (marigold_pipeline.py:237-247).  torchvision resizes a uint8 tensor as a float resize
+        # followed by clamp (bicubic) and round back to uint8: normalise_rgb(round_u8) does both.
         was_u8 = rgb.dtype == torch.uint8
         rgb = rgb.to(self.device)
         rgb = rgb.to(torch.float32)                        # dtype cast at the API boundary
         if processing_res > 0:
-            rgb = _resize_max_res(rgb, processing_res)
+            rgb = _resize_max_res(rgb, processing_res, resample_method)
         rgb_norm = normalise_rgb(rgb, round_u8=was_u8 and processing_res > 0)
         lo, hi = minmax_rows(rgb_norm.view(1, -1))[0].tolist()
         assert lo >= -1.0 and hi <= 1.0
@@ -394,6 +421,14 @@ class MarigoldPipeline(PipelineBase):
                 pred, pred_uncert = ensemble_depths(preds, **(ensemble_kwargs or {}))
         else:
             pred = preds
+        return self._postprocess(pred, pred_uncert, tuple(input_size[-2:]), normals=normals,
+                                 match_input_res=match_input_res, resample_method=resample_method, color_map=color_map)
+
+    def _postprocess(self, pred, pred_uncert, input_hw, normals=False, match_input_res=True,
+                     resample_method="bilinear", color_map="Spectral") -> MarigoldDepthOutput:
+        """marigold_pipeline.py:298-350 on the device, from the (ensembled) prediction to the output: unit normals or
+        [0, 1] depth, resize back with the call's resampling, one copy to the host, clip; the colour image is built
+        by a kernel from the same device tensor and copied to the host once as uint8."""
         pred = pred.to(torch.float32).contiguous()
         if normals:
             pred = ops.decode_post(pred[None], normals=True)[0]            # pred / (|pred| + 1e-5)   (:300-303)
@@ -403,15 +438,19 @@ class MarigoldPipeline(PipelineBase):
             if hi == lo:
                 pred = torch.zeros_like(pred)
         if match_input_res:
-            pred = resize_bilinear_aa(pred if normals else pred.unsqueeze(0),
-                                      (input_size[-2], input_size[-1])).squeeze()
+            pred = _resize(pred if normals else pred.unsqueeze(0), input_hw, resample_method).squeeze()
+        # colours of the clipped map (:327-343): the kernels clip as numpy does, so they read the same device tensor
+        if normals:
+            colored = _to_pil(colorize_normals(pred))
+        else:
+            colored = None if color_map is None else _to_pil(colorize_depth(pred, color_map))
         pred = pred.cpu().numpy()
         if pred_uncert is not None:
             pred_uncert = pred_uncert.cpu().numpy() if torch.is_tensor(pred_uncert) else pred_uncert
         pred = pred.clip(-1.0, 1.0) if normals else pred.clip(0, 1)
-        # colourising needs matplotlib (absent): the color_map=None path of marigold_pipeline.py:330-338
-        return MarigoldDepthOutput(depth_np=None if normals else pred, depth_colored=None, uncertainty=pred_uncert,
-                                   normal_np=pred if normals else None, normal_colored=None)
+        return MarigoldDepthOutput(depth_np=None if normals else pred, depth_colored=None if normals else colored,
+                                   uncertainty=pred_uncert, normal_np=pred if normals else None,
+                                   normal_colored=colored if normals else None)
 
     def encode_empty_text(self):
         if self.text_encoder is None:
@@ -658,8 +697,9 @@ class DepthNormalEstimationPipeline(PipelineBase):
     def __call__(self, input_image, denoising_steps: int = 1, ensemble_size: int = 1, processing_res: int = 768,
                  match_input_res: bool = True, domain: str = "indoor", color_map: Optional[str] = None,
                  show_progress_bar: bool = False, noise="zeros", img_embed=None,
-                 batch_size: int = 0) -> DepthNormalPipelineOutput:
+                 batch_size: int = 0, ensemble_kwargs=None) -> DepthNormalPipelineOutput:
         _check_geowizard_noise(noise, denoising_steps)
+        check_color_map(color_map)
         assert ensemble_size >= 1 and batch_size >= 0
         if isinstance(input_image, torch.Tensor):
             rgb = input_image.squeeze()
@@ -682,7 +722,7 @@ class DepthNormalEstimationPipeline(PipelineBase):
         depth, normal = torch.cat(dl).squeeze(), torch.cat(nl).squeeze()
         uncert = None
         if ensemble_size > 1:                               # :179-188
-            depth, uncert = ensemble_depths(depth)
+            depth, uncert = ensemble_depths(depth, **(ensemble_kwargs or {}))
             normal, _ = ensemble_normals(normal)
         depth, _ = minmax_normalise_(depth.to(torch.float32).contiguous())      # :192-194
         normal = normal.to(torch.float32)
@@ -690,6 +730,9 @@ class DepthNormalEstimationPipeline(PipelineBase):
             # the reference resizes on the host (PIL for depth, cv2 INTER_NEAREST for normals, :201-206); here on the device
             depth = resize_bilinear_aa(depth[None], tuple(input_size[-2:]))[0]
             normal = resize_nearest(normal, tuple(input_size[-2:]))
-        return DepthNormalPipelineOutput(depth_np=depth.cpu().numpy().clip(0, 1), depth_colored=None,
-                                         normal_np=normal.cpu().numpy().clip(-1, 1), normal_colored=None,
+        # colours (:210-220) from the device tensors that become depth_np / normal_np; the kernels clip as numpy does
+        depth_colored = None if color_map is None else _to_pil(colorize_depth(depth, color_map))
+        normal_colored = _to_pil(colorize_normals(normal))
+        return DepthNormalPipelineOutput(depth_np=depth.cpu().numpy().clip(0, 1), depth_colored=depth_colored,
+                                         normal_np=normal.cpu().numpy().clip(-1, 1), normal_colored=normal_colored,
                                          uncertainty=None if uncert is None else uncert.cpu().numpy())

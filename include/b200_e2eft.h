@@ -347,6 +347,21 @@ int b200_resize_bilinear_aa(const float* x, long long planes, int H, int W, int 
                             void* stream);
 int b200_resize_nearest(const float* x, long long planes, int H, int W, int OH, int OW, float* out, void* stream);
 
+/* Resampling choice and colour outputs of the pipelines' __call__ (ABI 9).
+ * b200_resize_nearest_exact: torch interpolate(mode="nearest-exact") of [planes][H][W] fp32 -> [planes][OH][OW],
+ *   src = min(floor((dst + 0.5) * (in / out)), in - 1) with the fp32 scale; the reference's resample_method="nearest"
+ *   (Marigold/marigold/util/image_util.py:111-116, marigold_pipeline.py:219,237-242,315-321).
+ * b200_colorize_depth: fp32 [n] -> uint8 [n][3] through table [ncol][3] uint8 (ncol <= 4096):
+ *   colorize_depth_maps(pred, 0, 1, cmap) then (colored * 255).astype(uint8) and chw2hwc
+ *   (Marigold/marigold/util/image_util.py:29-67, marigold_pipeline.py:327-338, geowizard_pipeline.py:211-216);
+ *   index (int)(clip(x, 0, 1) * ncol) with ncol -> ncol - 1, NaN -> (0, 0, 0); out 4-byte aligned.
+ * b200_colorize_normals: fp32 [3][HW] -> uint8 [HW][3] = ((clip(x, -1, 1) + 1) / 2 * 255) truncated, NaN -> 0
+ *   (marigold_pipeline.py:339-343, geowizard_pipeline.py:218-219); out 4-byte aligned. */
+int b200_resize_nearest_exact(const float* x, long long planes, int H, int W, int OH, int OW, float* out, void* stream);
+int b200_colorize_depth(const float* x, long long n, const unsigned char* table, int ncol, unsigned char* out,
+                        void* stream);
+int b200_colorize_normals(const float* x, long long HW, unsigned char* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
