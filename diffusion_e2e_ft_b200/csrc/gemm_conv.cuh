@@ -11,10 +11,17 @@
 //   Optional second source A2 (same pixel tiling, 1x1) appends k-blocks: this fuses the
 //   ResnetBlock2D 1x1 `conv_shortcut` into conv2's accumulation.
 // * Two consumer warpgroups (warps 0-7) each issue wgmma m64nBLOCK_Nk16 for one 64-row half of the 128-row tile,
-//   accumulating in registers; warp 8 is the TMA producer.  After the main loop of a tile the accumulators are
-//   staged as fp32 into the (then idle) operand ring and the same 8 warps run the epilogue from there: thread
-//   (warp & 3, lane) owns accumulator row 32 (warp & 3) + lane, the two warps of a row quadrant take alternate
-//   32-column chunks.  The producer starts the next tile's loads once every epilogue thread has released the ring.
+//   accumulating in registers; warps 8-11 are the producer warpgroup, of which one lane issues the TMA loads.  The
+//   producer warpgroup gives up registers (setmaxnreg.dec 40) so the consumers can hold the 128 accumulator registers
+//   of a 256-wide tile plus the epilogue's working set without spilling (setmaxnreg.inc 232).
+// * Epilogue, vectorised swapped orientation (VEC): straight from the accumulator registers.  Each warp owns 16 rows
+//   (channels) of the tile and turns them, 32 columns (pixels) at a time, into per-pixel channel runs through a small
+//   per-warp smem tile.  No CTA barrier and no use of the operand ring, so the producer fills the ring with the next
+//   tile's operands while the epilogue runs.
+// * Epilogue, every other instantiation: the accumulators are staged as fp32 into the (then idle) operand ring and the
+//   same 8 warps run the epilogue from there: thread (warp & 3, lane) owns accumulator row 32 (warp & 3) + lane, the two
+//   warps of a row quadrant take alternate 32-column chunks.  The producer starts the next tile's loads once every
+//   epilogue thread has released the ring.
 // * Persistent: grid = min(#tiles, #SMs), static round-robin tile schedule (n fastest).
 #pragma once
 #include <type_traits>
@@ -27,9 +34,12 @@ namespace b200 {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;       // 64 x fp16 = one 128-byte swizzle row
 constexpr int kMmaK = 16;
-constexpr int kGemmThreads = 288;   // warps 0-7: two MMA + epilogue warpgroups, warp 8: TMA producer
+constexpr int kGemmThreads = 384;   // warps 0-7: two MMA + epilogue warpgroups, warps 8-11: producer warpgroup
 constexpr int kEpiWarps = 8;
 constexpr int kConsumerThreads = 32 * kEpiWarps;
+// per-thread register budgets after the role split: 128 * 40 + 256 * 232 <= 384 * 168 (the launch allocation)
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
 constexpr int kMaxTaps = 9;
 
 enum EpiAct { ACT_NONE = 0, ACT_SILU = 1, ACT_GEGLU = 2, ACT_GELU = 3, ACT_EXP2 = 4 };   // EXP2: P = exp2(alpha S - lse)
@@ -77,7 +87,9 @@ struct GemmParams {
   int debug;                   // perf experiments: 1 = no epilogue stores, 2 = no A loads, 4 = no B loads, 8 = no MMAs, 16 = empty epilogue
 };
 
-constexpr int kSwapPitch = 36;      // floats per row of the swapped epilogue's transpose tile (16-byte aligned, conflict-free)
+// floats per pixel row of the vectorised epilogue's per-warp [32 pixels][16 channels] transpose tile: 16-byte aligned,
+// and 20 makes both the fragment stores and the 16-byte pixel-row loads bank-conflict-free
+constexpr int kSwapPitch = 20;
 
 // HALO (conv3x3, stride 1, swapped orientation): the activation patch of a tile — (bh+2) x (bw+2) pixels x 64 channels —
 // is loaded ONCE per 64-channel block and all nine taps are issued as row-shifted views of it (wgmma descriptors with a
@@ -262,8 +274,11 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
   __syncthreads();
 
-  if (warp == kEpiWarps) {
+  if (warp >= kEpiWarps) {
     // ======================================================================= TMA producer
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kProducerRegs));
+    if (warp != kEpiWarps) return;
+    // VEC epilogues never touch the ring, so only the staged epilogues hold the producer back at a tile boundary
     uint32_t aphase = 0;
     if constexpr (HALO) {
       if (lane == 0) {
@@ -278,8 +293,10 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const int th = r2 % p.tiles_h;
           const int img = r2 / p.tiles_h;
           const int h0 = th * p.bh, w0 = tw * p.bw;
-          mbar_wait(acc_empty, aphase ^ 1);                  // the accumulators of the previous tile left the ring
-          aphase ^= 1;
+          if constexpr (!VEC) {
+            mbar_wait(acc_empty, aphase ^ 1);                // the accumulators of the previous tile left the ring
+            aphase ^= 1;
+          }
           for (int blk = 0; blk < p.cin_blocks + p.k2_blocks; ++blk) {
             const bool main = blk < p.cin_blocks;
             mbar_wait(&patch_empty[pb], pphase ^ 1);
@@ -325,8 +342,10 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           h0 = th * p.bh;
           w0 = tw * p.bw;
         }
-        mbar_wait(acc_empty, aphase ^ 1);                    // the accumulators of the previous tile left the ring
-        aphase ^= 1;
+        if constexpr (!VEC) {
+          mbar_wait(acc_empty, aphase ^ 1);                  // the accumulators of the previous tile left the ring
+          aphase ^= 1;
+        }
         for (int kb = 0; kb < p.num_k_blocks; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           mbar_arrive_expect_tx(&full_bar[stage], ((p.debug & 2) ? 0u : a_bytes) + ((p.debug & 4) ? 0u : b_bytes));
@@ -374,13 +393,13 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
   } else {
     // ======================================================================= MMA + epilogue warpgroups
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kConsumerRegs));
     const int wg = warp >> 2;                        // MMA rows 64 wg .. 64 wg + 63 of the 128-row tile
     int stage = 0, ws = 0, pb = 0;
     uint32_t phase = 0, wphase = 0, pphase = 0;
-    // Main loop of this CTA's next tile; returns with the fp32 accumulators in acc_smem (row-major, kAccPitch).
+    // Main loop of this CTA's next tile; returns with this warpgroup's fp32 accumulators in d (layout in wgmma.cuh).
     // One k-block of MMAs stays in flight: a ring slot is released once the MMAs after it have been issued.
-    auto mma_tile = [&]() {
-      float d[BLOCK_N / 2];
+    auto mma_main = [&](float (&d)[BLOCK_N / 2]) {
 #pragma unroll
       for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
       if constexpr (HALO) {
@@ -458,6 +477,11 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_fence_operands<BLOCK_N / 2>(d);
         mbar_arrive(&empty_bar[prev]);
       }
+    };
+    // Main loop of this CTA's next tile; returns with the fp32 accumulators in acc_smem (row-major, kAccPitch).
+    auto mma_tile = [&]() {
+      float d[BLOCK_N / 2];
+      mma_main(d);
       // both warpgroups' MMAs have retired (they read the ring) before it is overwritten with the accumulators
       asm volatile("bar.sync 1, 256;" ::: "memory");
       {
@@ -503,7 +527,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       int scnt = 0;
       long long skey = -1;                                         // (image * N + first channel) the sums belong to
       auto flush_stats = [&]() {
-        // plain sums in fp64 (each lane has its own shift), folded over the four lanes that share a channel quad
+        // plain sums in fp64 (each lane has its own shift), folded over the eight lanes that share a channel quad
+        // (lane & 3 = quad, see the vectorised epilogue below)
         double d1[4], d2[4];
         const double n = (double)scnt;
 #pragma unroll
@@ -511,12 +536,13 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const double shd = (double)sh[k], a = (double)s1[k];
           d1[k] = a + n * shd;
           d2[k] = (double)s2[k] + 2.0 * shd * a + n * shd * shd;
-          d1[k] += __shfl_xor_sync(0xffffffffu, d1[k], 8);
-          d2[k] += __shfl_xor_sync(0xffffffffu, d2[k], 8);
-          d1[k] += __shfl_xor_sync(0xffffffffu, d1[k], 16);
-          d2[k] += __shfl_xor_sync(0xffffffffu, d2[k], 16);
+#pragma unroll
+          for (int m = 4; m < 32; m <<= 1) {
+            d1[k] += __shfl_xor_sync(0xffffffffu, d1[k], m);
+            d2[k] += __shfl_xor_sync(0xffffffffu, d2[k], m);
+          }
         }
-        if ((lane >> 3) == 0 && skey >= 0) {
+        if ((lane >> 2) == 0 && skey >= 0) {
           double* dst = p.chan_stats + skey * 2;
 #pragma unroll
           for (int k = 0; k < 4; ++k) {
@@ -602,14 +628,16 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
         if constexpr (VEC) {
           // ---------------------------------------------------------------- vectorised path (16-byte accesses)
-          // The staged row hands each lane ONE channel of 32 pixels; NHWC wants, per pixel, runs of consecutive channels.  Each
-          // 32x32 chunk goes through a per-warp smem tile (STS.32 by pixel row, LDS.128 back): afterwards lane
-          // (pr = lane / 8, q = lane % 8) owns channels 4q..4q+3 of pixels pr, pr+4, ..., pr+28, so residual loads /
-          // output stores are 16-byte (fp32) or 8-byte (fp16) accesses, four 128-byte pixel rows per warp instruction
-          // — a quarter of the memory instructions of the scalar path.
-          float* stgw = reinterpret_cast<float*>(stage_smem + S::kSwapTabBytes) + ew * (32 * kSwapPitch);
-          const int q = lane & 7, pr = lane >> 3;
-          const int chq = n_blk * kBlockM + quad * 32 + 4 * q;          // first of this lane's four channels
+          // Straight from the accumulator registers: warp w holds tile rows (channels) 16 w .. 16 w + 15 for all columns
+          // (pixels), lane l two channels of column pairs (wgmma.cuh).  NHWC wants, per pixel, runs of consecutive
+          // channels, so each 16 x 32 chunk goes through the warp's [32 pixels][kSwapPitch] smem tile (STS.32 from the
+          // fragment, LDS.128 back): afterwards lane (pr, q = lane % 4) owns channels 4q..4q+3 of pixels pr, pr+8, pr+16,
+          // pr+24, and each residual load / output store moves 16 bytes (fp32) or 8 bytes (fp16) per lane — eight
+          // 64-byte (fp32) or 32-byte (fp16) pixel runs of whole sectors per warp instruction.  pr pairs pixels p and
+          // p + 4 in every group of 8 lanes, which keeps the 16-byte loads conflict-free at pitch 20.
+          float* stgw = reinterpret_cast<float*>(stage_smem + S::kSwapTabBytes) + warp * (32 * kSwapPitch);
+          const int q = lane & 3, pr = (lane >> 3) + 4 * ((lane >> 2) & 1);
+          const int chq = n_blk * kBlockM + warp * 16 + 4 * q;          // first of this lane's four channels
           const bool cq_ok = chq < p.N;                                 // N % 4 == 0 on this path
           float add4[4] = {0.f, 0.f, 0.f, 0.f};
           if (cq_ok) {
@@ -636,40 +664,44 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           const OutT* __restrict__ res_q = res ? res + (long long)b * p.res_batch_stride + pix0 * p.ld_res + chq : nullptr;
           __half* __restrict__ out2_q = p.out2 ? p.out2 + (long long)b * p.out_batch_stride + pix0 * p.ldo + chq : nullptr;
           using Vec = typename std::conditional<std::is_same<OutT, float>::value, float4, uint2>::type;
-          if (p.chan_stats) {
-            // warp-uniform: every lane of the warp switches key on the same tile (invalid channel quads keep key -1)
-            const long long key_w = (long long)img * p.N + n_blk * kBlockM + quad * 32;
-            const long long key = cq_ok ? key_w + 4 * q : -1;
-            const long long cur_w = __shfl_sync(0xffffffffu, skey >= 0 ? skey - 4 * q : -1, 0);
-            if (cur_w != key_w && __any_sync(0xffffffffu, scnt > 0)) flush_stats();
-            skey = key;
-          }
-          mma_tile();
+          if (p.chan_stats) skey = cq_ok ? (long long)img * p.N + chq : -1;   // invalid channel quads keep key -1
+          float frag[BLOCK_N / 2];
+          mma_main(frag);
           // conv tiles may use fewer than BLOCK_N accumulator columns (bw * bh pixels)
           const int ncols = p.conv ? min(BLOCK_N, (p.col_pitch * p.bh + 31) & ~31) : BLOCK_N;
           if (!(p.debug & 16)) {
-#pragma unroll 1
-            for (int c = eg * 32; c < ncols; c += 64) {
-              uint32_t oo[8];
-              Vec rres[8];
+            // unrolled over the chunks: every fragment register index is then a compile-time constant (a loop-carried
+            // index would move frag to local memory)
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const uint32_t dd = s_dhdw[c + 4 * i + pr];
+            for (int c = 0; c < BLOCK_N; c += 32) {
+              if (c >= ncols) break;
+              uint32_t oo[4];
+              Vec rres[4];
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const uint32_t dd = s_dhdw[c + 8 * i + pr];
                 const bool ok = cq_ok && (int)(dd >> 16) < lim_h && (int)(dd & 0xFFFFu) < lim_w;
-                oo[i] = ok ? s_rel_out[c + 4 * i + pr] : 0xFFFFFFFFu;
+                oo[i] = ok ? s_rel_out[c + 8 * i + pr] : 0xFFFFFFFFu;
               }
-              if (res_q != nullptr) {                // residual rows first: their latency hides behind the accumulator read
+              if (res_q != nullptr) {                // residual rows first: their latency hides behind the transpose
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
-                  if (oo[i] != 0xFFFFFFFFu) rres[i] = *reinterpret_cast<const Vec*>(res_q + s_rel_res[c + 4 * i + pr]);
+                for (int i = 0; i < 4; ++i)
+                  if (oo[i] != 0xFFFFFFFFu) rres[i] = *reinterpret_cast<const Vec*>(res_q + s_rel_res[c + 8 * i + pr]);
               }
-              uint32_t r[32];
-              acc_ld(t_row + c, r);
+              // fragment columns c .. c + 31 (frag[4j .. 4j + 3], j = c / 8 .. c / 8 + 3) into the tile: pixel
+              // 8 (j % 4) + 2 (lane % 4) + {0, 1}, channel lane / 4 + {0, 8}
 #pragma unroll
-              for (int j = 0; j < 32; ++j) stgw[j * kSwapPitch + lane] = __uint_as_float(r[j]);
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = c / 8 + jj;
+                float* dst = stgw + (8 * jj + 2 * (lane & 3)) * kSwapPitch + (lane >> 2);
+                dst[0] = frag[4 * j];
+                dst[kSwapPitch] = frag[4 * j + 1];
+                dst[8] = frag[4 * j + 2];
+                dst[kSwapPitch + 8] = frag[4 * j + 3];
+              }
               __syncwarp();
-              // phase A: accumulator * alpha + bias (+ residual) for the lane's 8 pixels x 4 channels
-              float v[8][4];
+              // phase A: accumulator * alpha + bias (+ residual) for the lane's 4 pixels x 4 channels
+              float v[4][4];
               auto res4 = [&](int i, float* r4) {          // the residual / multiplicative operand of pixel i as fp32
                 if constexpr (std::is_same<OutT, float>::value) {
                   r4[0] = rres[i].x; r4[1] = rres[i].y; r4[2] = rres[i].z; r4[3] = rres[i].w;
@@ -680,8 +712,8 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
                 }
               };
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 t4 = *reinterpret_cast<const float4*>(stgw + (4 * i + pr) * kSwapPitch + 4 * q);
+              for (int i = 0; i < 4; ++i) {
+                const float4 t4 = *reinterpret_cast<const float4*>(stgw + (8 * i + pr) * kSwapPitch + 4 * q);
                 v[i][0] = fmaf(t4.x, p.alpha, add4[0]); v[i][1] = fmaf(t4.y, p.alpha, add4[1]);
                 v[i][2] = fmaf(t4.z, p.alpha, add4[2]); v[i][3] = fmaf(t4.w, p.alpha, add4[3]);
                 if (res_q != nullptr && !p.res_mul && oo[i] != 0xFFFFFFFFu) {
@@ -695,18 +727,18 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               // interleaved into the unrolled pixel loop bloat it with instruction-fetch stalls)
               if (p.act == ACT_SILU) {
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
+                for (int i = 0; i < 4; ++i)
 #pragma unroll
                   for (int k = 0; k < 4; ++k) v[i][k] = silu_f(v[i][k]);
               } else if (p.act == ACT_GELU) {
 #pragma unroll
-                for (int i = 0; i < 8; ++i)
+                for (int i = 0; i < 4; ++i)
 #pragma unroll
                   for (int k = 0; k < 4; ++k) v[i][k] = gelu_erf_f(v[i][k]);
               }
               // phase C: multiplicative operand, stores, statistics
 #pragma unroll
-              for (int i = 0; i < 8; ++i) {
+              for (int i = 0; i < 4; ++i) {
                 const bool ok = oo[i] != 0xFFFFFFFFu;
                 if (res_q != nullptr && p.res_mul && ok) {
                   float r4[4];
@@ -748,8 +780,19 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
               __syncwarp();                          // the tile is rewritten by the next chunk
             }
           }
-          release_acc();
-          acc ^= 1;
+          if (p.chan_stats) {
+            // merge the carried sums when this CTA's next tile belongs to another (image, channel tile), or at its last
+            // tile (warp-uniform).  Flushing here rather than after the tile loop keeps the whole consumer path inside
+            // the setmaxnreg.inc region, where ptxas allocates up to kConsumerRegs.
+            const int nt = tile + gridDim.x;
+            bool same = false;
+            if (nt < total_tiles) {
+              const int nn = nt % p.n_tiles, nm = (nt / p.n_tiles) % p.m_tiles;
+              const int nimg = p.conv ? nm / p.tiles_w / p.tiles_h : (int)(((long long)nm * BLOCK_N) / p.rows_per_img);
+              same = nn == n_blk && nimg == img;
+            }
+            if (!same && __any_sync(0xffffffffu, scnt > 0)) flush_stats();
+          }
           continue;
         }
         mma_tile();
@@ -837,7 +880,6 @@ gemm_conv_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         release_acc();
         acc ^= 1;
       }
-      if (VEC && p.chan_stats && __any_sync(0xffffffffu, scnt > 0)) flush_stats();
     } else {
     float (*stg)[33] = reinterpret_cast<float (*)[33]>(stage_smem + ew * (32 * 33 * 4));
     // per-warp row tables (16-byte aligned): element offsets of each of the warp's 32 rows relative to the

@@ -1,11 +1,71 @@
 """Tiny launcher for ncu captures of single kernels at production shapes.
-    python tools/prof_kernels.py conv128|conv320|conv1280|attn|gn|linear"""
+    python tools/prof_kernels.py conv128|conv320|conv1280|attn|gn|linear
+    python tools/prof_kernels.py vae [reps]   -- the VAE's hot convs as the model calls them (modules.py ResnetBlock2D /
+                                                 Upsample2D, batch 8 at 768^2), each timed with the debug flags
+                                                 0 (full), 16 (empty epilogue), 1 (no stores) and 8 (no MMAs)"""
 import os, sys, math
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 from diffusion_e2e_ft_b200 import ops
 what = sys.argv[1]
+
+
+def _vae_attribution(reps):
+    L = ops._lib.load()
+    g = torch.Generator(device="cpu").manual_seed(0)
+    rnd = lambda *s, sc=1.0, dt=torch.float16: (torch.randn(*s, generator=g) * sc).to(dt).to("cuda")
+    NB = 8
+    cases = []     # (name, fn, flops)
+    for H, C in ((768, 128), (384, 256), (192, 512)):
+        x16 = rnd(NB, H, H, C)
+        x32 = rnd(NB, H, H, C, dt=torch.float32)
+        w = ops.pack_conv(rnd(C, C, 3, 3, sc=1 / math.sqrt(9 * C)))
+        b = torch.zeros(C, device="cuda")
+        fl = 2 * NB * H * H * C * 9 * C
+        cases.append((f"conv1 {C}@{H} f16+stats", lambda x=x16, w=w, b=b, C=C: ops.conv2d(x, w, C, bias=b, stats=True), fl))
+        cases.append((f"conv2 {C}@{H} f32+res+stats+f16copy",
+                      lambda x=x16, w=w, b=b, C=C, r=x32: ops.conv2d(x, w, C, bias=b, residual=r, out_dtype=torch.float32,
+                                                                      stats=True, f16_copy=True), fl))
+    # shortcut conv2 (256 -> 128 at 768^2: decoder up-block 3, first resnet) and the 4-phase upsample (256 ch, 384 -> 768)
+    xs = rnd(NB, 768, 768, 128); x2 = rnd(NB, 768, 768, 256)
+    ws = ops.pack_conv(rnd(128, 128, 3, 3, sc=1 / math.sqrt(1152)), rnd(128, 256, 1, 1, sc=1 / 16))
+    bs = torch.zeros(128, device="cuda")
+    cases.append(("conv2 128@768 shortcut x2 f32+stats",
+                  lambda: ops.conv2d(xs, ws, 128, bias=bs, x2=x2, out_dtype=torch.float32, stats=True, f16_copy=True),
+                  2 * NB * 768 * 768 * 128 * (1152 + 256)))
+    from diffusion_e2e_ft_b200.modules import Upsample2D
+    up = Upsample2D(256).cuda()
+    xu = rnd(NB, 384, 384, 256, dt=torch.float32)
+    cases.append(("upsample 256@384->768 4-phase", lambda: up.run(xu, None, torch.float32),
+                  2 * NB * 768 * 768 * 256 * 4 * 256))
+    flags = (0, 16, 1, 8)
+    print(f"{'shape':42s} " + " ".join(f"{'flag ' + str(f):>10s}" for f in flags) + "   TFLOP/s")
+    with torch.no_grad():
+        for name, fn, fl in cases:
+            ms = []
+            for f in flags:
+                L.b200_debug_set_flags(f)
+                try:
+                    for _ in range(2):
+                        fn()
+                    torch.cuda.synchronize()
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(reps):
+                        fn()
+                    e1.record(); torch.cuda.synchronize()
+                finally:
+                    L.b200_debug_set_flags(0)
+                ms.append(e0.elapsed_time(e1) / reps)
+            print(f"{name:42s} " + " ".join(f"{m:8.3f}ms" for m in ms) + f"   {fl / ms[0] / 1e9:7.1f}")
+
+
+if what == "vae":
+    if os.environ.get("B200_HALO"):      # 2: halo path even where the dispatcher calls the conv epilogue-bound
+        ops._lib.load().b200_debug_set_halo(int(os.environ["B200_HALO"]))
+    _vae_attribution(int(sys.argv[2]) if len(sys.argv) > 2 else 10)
+    sys.exit(0)
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 from diffusion_e2e_ft_b200 import lib as _l
 if len(sys.argv) > 3:
