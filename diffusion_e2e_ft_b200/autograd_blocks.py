@@ -629,21 +629,23 @@ class _PointwiseFn(torch.autograd.Function):
     """Conv1x1Small (post_quant_conv with the x0 / scaling-factor coefficients folded in): out = W (a1 * x) + b."""
 
     @staticmethod
-    def forward(ctx, conv, a1, x):
+    def forward(ctx, conv, a1, x, const=None, a2=0.0):
         w = conv.weight.detach().reshape(conv.out_channels, conv.in_channels).to(F32).contiguous()
         b = conv.bias.detach().to(F32).contiguous()
         ctx.w, ctx.a1 = w, a1
-        return ops.pointwise_nchw(x.float().contiguous(), a1, w, b, cin=conv.in_channels)
+        c = None if const is None else const.detach().float().contiguous()
+        return ops.pointwise_nchw(x.float().contiguous(), a1, w, b, in2=c, a2=a2, cin=conv.in_channels)
 
     @staticmethod
     def backward(ctx, dout):
         wt = ctx.w.t().contiguous()
         zero = torch.zeros((wt.shape[0],), dtype=F32, device=dout.device)
-        return None, None, ops.pointwise_nchw(dout.float().contiguous(), ctx.a1, wt, zero, cin=wt.shape[1])
+        return None, None, ops.pointwise_nchw(dout.float().contiguous(), ctx.a1, wt, zero, cin=wt.shape[1]), None, None
 
 
-def pointwise(conv, x, a1):
-    return _PointwiseFn.apply(conv, a1, x)
+def pointwise(conv, x, a1, const=None, a2=0.0):
+    """W (a1 * x + a2 * const) + b; `const` (e.g. the noisy latent x_t of a noisy-start step) carries no gradient."""
+    return _PointwiseFn.apply(conv, a1, x, const, a2)
 
 
 class _DecodePostFn(torch.autograd.Function):
@@ -677,3 +679,24 @@ class _LossFn(torch.autograd.Function):
 
 def task_loss(est, target, mask, normals):
     return _LossFn.apply(est, target, mask, normals)
+
+
+class _MaskedLatentMSEFn(torch.autograd.Function):
+    """Diffusion-objective loss (train_depth_normal.py:607-609,712-714): the latent mask is pooled from the pixel mask
+    once, in the forward, and saved with the fp64 (sum, count) workspace for the backward."""
+
+    @staticmethod
+    def forward(ctx, pred, target, val_mask):
+        pred = pred.contiguous()
+        loss, lm, ws = ops.masked_latent_mse(pred, target, val_mask)
+        ctx.saved = (pred, target, lm, ws)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gout):
+        pred, target, lm, ws = ctx.saved
+        return ops.masked_latent_mse_bwd(pred, target, lm, ws, gout), None, None
+
+
+def masked_latent_mse(pred, target, val_mask):
+    return _MaskedLatentMSEFn.apply(pred, target.detach(), val_mask)

@@ -17,19 +17,33 @@ WEIGHTS_BIN = "diffusion_pytorch_model.bin"
 CONFIG_NAME = "config.json"
 
 
+def load_weights(directory):
+    """The state dict of a diffusers model folder (safetensors, else .bin), on the CPU."""
+    safe, binp = os.path.join(directory, WEIGHTS_SAFE), os.path.join(directory, WEIGHTS_BIN)
+    if os.path.exists(safe):
+        from safetensors.torch import load_file
+        return load_file(safe)
+    if os.path.exists(binp):
+        return torch.load(binp, map_location="cpu")
+    raise FileNotFoundError(f"no {WEIGHTS_SAFE} / {WEIGHTS_BIN} in {directory}")
+
+
 class PretrainedMixin:
     _diffusers_class_name = None       # e.g. "UNet2DConditionModel"
     _config_defaults = None            # dict of the keys the engine models
 
-    def save_pretrained(self, save_directory, safe_serialization=True, **unused):
+    def save_pretrained(self, save_directory, safe_serialization=True, state_dict=None, extra_config=None, **unused):
+        """`state_dict`: weights to write instead of the module's own (e.g. an EMA copy, same names and shapes);
+        `extra_config`: keys added to config.json (e.g. EMAModel's settings)."""
         os.makedirs(save_directory, exist_ok=True)
         cfg = {k: (list(v) if isinstance(v, tuple) else v) for k, v in self.config.items() if k != "_extra"}
         cfg.update(self.config.get("_extra", {}))
+        cfg.update(extra_config or {})
         cfg["_class_name"] = self._diffusers_class_name
         cfg.setdefault("_diffusers_version", "0.30.2")
         with open(os.path.join(save_directory, CONFIG_NAME), "w") as f:
             json.dump(cfg, f, indent=2, sort_keys=True)
-        sd = {k: v.detach().to("cpu").contiguous() for k, v in self.state_dict().items()}
+        sd = {k: v.detach().to("cpu").contiguous() for k, v in (state_dict or self.state_dict()).items()}
         if safe_serialization:
             from safetensors.torch import save_file
             save_file(sd, os.path.join(save_directory, WEIGHTS_SAFE), metadata={"format": "pt"})
@@ -63,15 +77,7 @@ class PretrainedMixin:
         model = cls(stream_dtype=stream, **known)
         if extra:
             model.config["_extra"] = extra
-        safe, binp = os.path.join(d, WEIGHTS_SAFE), os.path.join(d, WEIGHTS_BIN)
-        if os.path.exists(safe):
-            from safetensors.torch import load_file
-            sd = load_file(safe)
-        elif os.path.exists(binp):
-            sd = torch.load(binp, map_location="cpu")
-        else:
-            raise FileNotFoundError(f"no {WEIGHTS_SAFE} / {WEIGHTS_BIN} in {d}")
-        model.load_state_dict(sd, strict=True)
+        model.load_state_dict(load_weights(d), strict=True)
         if torch_dtype is not None:
             model = model.to(torch_dtype)
         return model.eval()

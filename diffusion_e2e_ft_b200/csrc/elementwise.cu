@@ -196,6 +196,31 @@ __global__ void ddim_step_kernel(const MO* __restrict__ mo, long long mo_bs, con
   }
 }
 
+// DDPM add_noise + get_velocity + the UNet-input concatenation of the diffusion objective, one pass over [2B][C][HW]:
+// unet_in[n] = [rgb[n mod B] | sqrt(a) x0 + sqrt(1-a) eps], target[n] = eps (epsilon) or sqrt(a) eps - sqrt(1-a) x0
+// (v_prediction), a = alphas_cumprod[t[n]].  Each product and sum rounded on its own, as torch evaluates diffusers'
+// expressions; eps = 0 when noise is null.
+__global__ void diffusion_inputs_kernel(const float* __restrict__ rgb, const float* __restrict__ x0,
+                                        const float* __restrict__ noise, const long long* __restrict__ t,
+                                        const float* __restrict__ ac, int B, long long CHW, int ptype,
+                                        float* __restrict__ unet_in, float* __restrict__ target) {
+  const int n = blockIdx.y;
+  const float a = ac[t[n]];
+  const float sa = __fsqrt_rn(a), sb = __fsqrt_rn(__fsub_rn(1.0f, a));
+  const float* xr = rgb + (long long)(n % B) * CHW;
+  const float* xb = x0 + (long long)n * CHW;
+  const float* nb = noise ? noise + (long long)n * CHW : nullptr;
+  float* ui = unet_in + (long long)n * 2 * CHW;
+  float* tg = target + (long long)n * CHW;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < CHW; i += (long long)gridDim.x * blockDim.x) {
+    const float x = xb[i];
+    const float e = nb ? nb[i] : 0.0f;
+    ui[i] = xr[i];
+    ui[CHW + i] = __fadd_rn(__fmul_rn(sa, x), __fmul_rn(sb, e));
+    tg[i] = ptype == B200_PRED_V ? __fsub_rn(__fmul_rn(sa, e), __fmul_rn(sb, x)) : e;
+  }
+}
+
 __global__ void cast_f32_f16_kernel(const float* __restrict__ x, __half* __restrict__ y, long long n) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n;
        i += (long long)gridDim.x * blockDim.x)
@@ -339,6 +364,24 @@ extern "C" int b200_ddim_step(const void* model_out, int mo_f16, long long mo_bs
   }
 #undef B200_DDIM
   B200_CHECK_LAUNCH("ddim_step_kernel");
+  return 0;
+}
+
+extern "C" int b200_diffusion_inputs(const float* rgb_latents, const float* x0, const float* noise,
+                                     const long long* timesteps, const float* alphas_cumprod, int B, int C,
+                                     long long HW, int prediction_type, float* unet_in, float* target,
+                                     void* stream) {
+  B200_CHECK_ARG(rgb_latents && x0 && timesteps && alphas_cumprod && unet_in && target,
+                 "b200_diffusion_inputs: null pointer");
+  B200_CHECK_ARG(B >= 1 && 2 * B <= 65535 && C >= 1 && HW >= 1, "b200_diffusion_inputs: bad shape B=%d C=%d HW=%lld",
+                 B, C, HW);
+  B200_CHECK_ARG(prediction_type == B200_PRED_EPSILON || prediction_type == B200_PRED_V,
+                 "b200_diffusion_inputs: prediction_type %d is not epsilon or v_prediction", prediction_type);
+  const long long CHW = (long long)C * HW;
+  dim3 grid(grid_for(CHW, 256), 2 * B);
+  diffusion_inputs_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(rgb_latents, x0, noise, timesteps, alphas_cumprod, B,
+                                                                  CHW, prediction_type, unet_in, target);
+  B200_CHECK_LAUNCH("diffusion_inputs_kernel");
   return 0;
 }
 

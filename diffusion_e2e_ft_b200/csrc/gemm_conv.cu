@@ -197,7 +197,7 @@ extern "C" void b200_debug_set_flags(int f) { b200::g_debug = f; }
 extern "C" void b200_debug_set_swap(int m) { b200::g_swap_mode = m; }
 extern "C" void b200_debug_set_halo(int m) { b200::g_halo_mode = m; }
 extern "C" int b200_debug_last_path(void) { return b200::g_last_path; }
-extern "C" int b200_abi_version(void) { return 9; }
+extern "C" int b200_abi_version(void) { return 10; }
 // Tile width used by the GEGLU epilogue for a packed width N (= 2 x output width); weights must be
 // packed per tile as [value half | gate half] with this width.
 extern "C" int b200_geglu_block_n(int N) {

@@ -73,6 +73,62 @@ __global__ void mean_finalize_kernel(const double* __restrict__ ws, float* __res
   out[0] = (float)(ws[0] / ws[1]);                            // empty mask -> nan, like torch's mean of an empty tensor
 }
 
+// Masked latent MSE of the diffusion objective (train_depth_normal.py:607-609,712-714).  One thread per latent pixel
+// (b, p): the pixel is valid iff all 64 pixels of its 8x8 block of val_mask are (~max_pool2d(~val_mask, 8, 8), floor
+// cropping); the mask is stored for the backward and, when valid, the squared differences of the 2 halves x C channels
+// of that pixel are summed in fp64.  ws[0] += sum, ws[1] += count (exact in fp64).
+template <typename T>
+__global__ void masked_latent_mse_kernel(const T* __restrict__ pred, const float* __restrict__ tgt,
+                                         const uint8_t* __restrict__ vm, int B, int C, int H, int W, int h, int w,
+                                         uint8_t* __restrict__ lm, double* __restrict__ ws) {
+  const int b = blockIdx.y;
+  const long long hw = (long long)h * w;
+  double acc = 0, cnt = 0;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
+    const int y = (int)(p / w), x = (int)(p - (long long)y * w);
+    const uint8_t* blk = vm + ((long long)b * H + 8 * y) * W + 8 * x;
+    bool ok = true;
+#pragma unroll
+    for (int r = 0; r < 8; ++r)
+#pragma unroll
+      for (int s = 0; s < 8; ++s) ok = ok && blk[(long long)r * W + s] != 0;
+    lm[(long long)b * hw + p] = ok;
+    if (ok) {
+      for (int half = 0; half < 2; ++half)
+        for (int c = 0; c < C; ++c) {
+          const long long idx = (((long long)half * B + b) * C + c) * hw + p;
+          const double d = (double)(float)pred[idx] - (double)tgt[idx];
+          acc += d * d;
+        }
+      cnt += 2.0 * C;
+    }
+  }
+  acc = warp_sum_d(acc); cnt = warp_sum_d(cnt);
+  if ((threadIdx.x & 31) == 0 && cnt > 0) { atomicAdd(&ws[0], acc); atomicAdd(&ws[1], cnt); }
+}
+
+__global__ void masked_mean_finalize_kernel(const double* __restrict__ ws, float* __restrict__ out) {
+  out[0] = ws[1] > 0 ? (float)(ws[0] / ws[1]) : 0.0f;          // empty mask: 0, not nan
+}
+
+// grad[n][c][p] = mask ? grad_out * 2 (pred - target) / count : 0, in pred's dtype
+template <typename T>
+__global__ void masked_latent_mse_bwd_kernel(const T* __restrict__ pred, const float* __restrict__ tgt,
+                                             const uint8_t* __restrict__ lm, const double* __restrict__ ws,
+                                             const float* __restrict__ grad_out, int B, int C, long long hw,
+                                             T* __restrict__ grad) {
+  const double cnt = ws[1];
+  const float s = cnt > 0 ? (float)(2.0 * (double)grad_out[0] / cnt) : 0.0f;
+  const long long total = 2LL * B * C * hw;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long p = i % hw;
+    const int b = (int)((i / (hw * C)) % B);
+    float g = 0.0f;
+    if (lm[(long long)b * hw + p]) g = __fmul_rn(s, __fsub_rn((float)pred[i], tgt[i]));
+    grad[i] = (T)g;
+  }
+}
+
 static dim3 loss_grid(long long HW, int B) {
   long long g = (HW + 256 * 8 - 1) / (256 * 8);
   long long cap = (long long)sm_count() * 4 / (B > 0 ? B : 1) + 1;
@@ -94,6 +150,46 @@ extern "C" int b200_ssi_loss(const float* pred, const float* target, const unsig
   ssi_l1_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, B, workspace);
   mean_finalize_kernel<<<1, 1, 0, st>>>(workspace + B * 5, out);
   B200_CHECK_LAUNCH("ssi_loss kernels");
+  return 0;
+}
+
+extern "C" int b200_masked_latent_mse(const void* pred, int pred_f16, const float* target, const unsigned char* val_mask,
+                                      int B, int C, int H, int W, int h, int w, unsigned char* latent_mask,
+                                      double* workspace, float* out, void* stream) {
+  B200_CHECK_ARG(pred && target && val_mask && latent_mask && workspace && out, "b200_masked_latent_mse: null pointer");
+  B200_CHECK_ARG(B >= 1 && B <= 65535 && C >= 1 && h >= 1 && w >= 1 && H >= 1 && W >= 1,
+                 "b200_masked_latent_mse: bad shape B=%d C=%d H=%d W=%d h=%d w=%d", B, C, H, W, h, w);
+  B200_CHECK_ARG(h == H / 8 && w == W / 8, "b200_masked_latent_mse: latent %dx%d is not the 8x8-pooled mask %dx%d",
+                 h, w, H / 8, W / 8);
+  cudaStream_t st = (cudaStream_t)stream;
+  dim3 grid = loss_grid((long long)h * w, B);
+  if (pred_f16)
+    masked_latent_mse_kernel<__half><<<grid, 256, 0, st>>>((const __half*)pred, target, val_mask, B, C, H, W, h, w,
+                                                           latent_mask, workspace);
+  else
+    masked_latent_mse_kernel<float><<<grid, 256, 0, st>>>((const float*)pred, target, val_mask, B, C, H, W, h, w,
+                                                          latent_mask, workspace);
+  masked_mean_finalize_kernel<<<1, 1, 0, st>>>(workspace, out);
+  B200_CHECK_LAUNCH("masked_latent_mse kernels");
+  return 0;
+}
+
+extern "C" int b200_masked_latent_mse_bwd(const void* pred, int pred_f16, const float* target,
+                                          const unsigned char* latent_mask, const double* workspace,
+                                          const float* grad_out, int B, int C, long long hw, void* grad, void* stream) {
+  B200_CHECK_ARG(pred && target && latent_mask && workspace && grad_out && grad, "b200_masked_latent_mse_bwd: null pointer");
+  B200_CHECK_ARG(B >= 1 && C >= 1 && hw >= 1, "b200_masked_latent_mse_bwd: bad shape");
+  const long long total = 2LL * B * C * hw;
+  long long g = (total + 255) / 256, cap = (long long)sm_count() * 16;
+  const unsigned blocks = (unsigned)(g < cap ? g : cap);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (pred_f16)
+    masked_latent_mse_bwd_kernel<__half><<<blocks, 256, 0, st>>>((const __half*)pred, target, latent_mask, workspace,
+                                                                 grad_out, B, C, hw, (__half*)grad);
+  else
+    masked_latent_mse_bwd_kernel<float><<<blocks, 256, 0, st>>>((const float*)pred, target, latent_mask, workspace,
+                                                                grad_out, B, C, hw, (float*)grad);
+  B200_CHECK_LAUNCH("masked_latent_mse_bwd_kernel");
   return 0;
 }
 

@@ -115,9 +115,37 @@ __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restric
     upd(p[i], g[i], m[i], v[i]);
 }
 
+// diffusers EMAModel.step: s_param.sub_(one_minus_decay * (s_param - param)), each operation rounded on its own.
+// 8 B read + 4 B written per parameter.
+__global__ void ema_update_kernel(float* __restrict__ ema, const float* __restrict__ p, long long n, float omd) {
+  const long long n4 = n / 4;
+  float4* e4 = reinterpret_cast<float4*>(ema);
+  const float4* p4 = reinterpret_cast<const float4*>(p);
+  auto upd = [&](float e, float q) { return __fsub_rn(e, __fmul_rn(omd, __fsub_rn(e, q))); };
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    float4 e = e4[i];
+    const float4 q = p4[i];
+    e.x = upd(e.x, q.x); e.y = upd(e.y, q.y); e.z = upd(e.z, q.z); e.w = upd(e.w, q.w);
+    e4[i] = e;
+  }
+  for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    ema[i] = upd(ema[i], p[i]);
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" int b200_ema_update(float* ema, const float* param, long long n, float one_minus_decay, void* stream) {
+  B200_CHECK_ARG(ema && param && n > 0, "b200_ema_update: bad arguments");
+  B200_CHECK_ARG((((uintptr_t)ema | (uintptr_t)param) & 15) == 0, "b200_ema_update: buffers must be 16-byte aligned");
+  long long g = (n / 4 + 255) / 256;
+  long long cap = (long long)sm_count() * 8;
+  ema_update_kernel<<<(unsigned)(g < 1 ? 1 : (g > cap ? cap : g)), 256, 0, (cudaStream_t)stream>>>(ema, param, n,
+                                                                                                    one_minus_decay);
+  B200_CHECK_LAUNCH("ema_update_kernel");
+  return 0;
+}
 
 extern "C" int b200_adamw_step_state(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
                                      float lr, float beta1, float beta2, float eps, float weight_decay,

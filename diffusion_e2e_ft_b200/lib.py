@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 9         # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 10        # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -88,6 +88,10 @@ _SIGS = {
     "b200_resize_nearest_exact": (c_int, [_P, _LL, c_int, c_int, c_int, c_int, _P, _P]),
     "b200_colorize_depth": (c_int, [_P, _LL, _P, c_int, _P, _P]),
     "b200_colorize_normals": (c_int, [_P, _LL, _P, _P]),
+    "b200_diffusion_inputs": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, _LL, c_int, _P, _P, _P]),
+    "b200_masked_latent_mse": (c_int, [_P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P]),
+    "b200_masked_latent_mse_bwd": (c_int, [_P, c_int, _P, _P, _P, _P, c_int, c_int, _LL, _P, _P]),
+    "b200_ema_update": (c_int, [_P, _P, _LL, c_float, _P]),
     "b200_cast_f32_to_f16": (c_int, [_P, _P, _LL, _P]),
     "b200_nhwc_to_nchw_f32": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P]),
 }

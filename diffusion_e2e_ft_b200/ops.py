@@ -801,3 +801,95 @@ def upsample_nearest_bwd(dy, in_hw, add=None):
     _ck(_lib.load().b200_upsample_nearest_bwd(_p(dy), NB, H, W, C, OH, OW, _p(add), _p(dx), _stream()),
         "b200_upsample_nearest_bwd")
     return dx
+
+
+# ------------------------------------------------------------------------------ diffusion objective + EMA (ABI 10)
+DIFFUSION_PREDICTION_TYPES = ("epsilon", "v_prediction")     # train_depth_normal.py:677-682
+
+
+@_timed("misc")
+def diffusion_inputs(rgb_latents, x0, noise, timesteps, alphas_cumprod, prediction_type, timesteps_host=None):
+    """DDPM add_noise + get_velocity + the UNet-input concatenation (train_depth_normal.py:666-705) in one kernel.
+    rgb_latents [B,C,h,w], x0 / noise [2B,C,h,w] fp32 (noise None = zeros), timesteps int64 [2B] on the device,
+    alphas_cumprod fp32 [T] on the device.  `timesteps_host`: the host copy of the timesteps for the range check (read
+    back from the device when omitted, a sync).  Returns (unet_in [2B,2C,h,w], target [2B,C,h,w]), both fp32."""
+    if prediction_type not in DIFFUSION_PREDICTION_TYPES:
+        raise ValueError(f"Unknown prediction type {prediction_type}")
+    _need_cuda(rgb_latents, x0, noise, timesteps, alphas_cumprod)
+    B, C, h, w = rgb_latents.shape
+    if tuple(x0.shape) != (2 * B, C, h, w) or (noise is not None and noise.shape != x0.shape):
+        raise ValueError(f"x0 / noise must be [2B, C, h, w] = {[2 * B, C, h, w]}, got {list(x0.shape)}"
+                         f"{'' if noise is None else ' / ' + str(list(noise.shape))}")
+    T = alphas_cumprod.numel()
+    th = [int(v) for v in (timesteps_host if timesteps_host is not None else timesteps.cpu()).reshape(-1).tolist()]
+    if len(th) != 2 * B or timesteps.numel() != 2 * B:
+        raise ValueError(f"timesteps must hold 2B = {2 * B} entries")
+    if not all(0 <= v < T for v in th):
+        raise ValueError(f"timesteps {th} outside [0, {T})")
+    for t in (rgb_latents, x0, noise, alphas_cumprod):
+        assert t is None or (t.dtype == F32 and t.is_contiguous())
+    assert timesteps.dtype == torch.long and timesteps.is_contiguous()
+    unet_in = torch.empty((2 * B, 2 * C, h, w), dtype=F32, device=x0.device)
+    target = torch.empty_like(x0)
+    _ck(_lib.load().b200_diffusion_inputs(_p(rgb_latents), _p(x0), _p(noise), _p(timesteps), _p(alphas_cumprod), B, C,
+                                          h * w, PREDICTION_TYPES[prediction_type], _p(unet_in), _p(target), _stream()),
+        "b200_diffusion_inputs")
+    return unet_in, target
+
+
+def latent_mask_shape(val_mask, pred):
+    """Checks that ~max_pool2d(~val_mask, 8, 8) has pred's spatial size and one image per pair of halves: the
+    reference's `noise_pred[latent_mask]` fails otherwise.  Returns (B, C, H, W, h, w)."""
+    if val_mask.dim() != 4 or val_mask.shape[1] != 1:
+        raise ValueError(f"val_mask must be [B, 1, H, W], got {list(val_mask.shape)}")
+    B, _, H, W = val_mask.shape
+    n, C, h, w = pred.shape
+    if n != 2 * B or (h, w) != (H // 8, W // 8):
+        raise ValueError(f"latent mask [{2 * B}, {C}, {H // 8}, {W // 8}] (max_pool2d 8x8 of val_mask {list(val_mask.shape)}) "
+                         f"does not match the prediction {list(pred.shape)}")
+    return B, C, H, W, h, w
+
+
+@_timed("loss")
+def masked_latent_mse(pred, target, val_mask):
+    """F.mse_loss(pred[latent_mask], target[latent_mask]) with latent_mask = ~max_pool2d(~val_mask, 8, 8) repeated over
+    both halves and all channels (train_depth_normal.py:607-609,712-714).  pred [2B,C,h,w] fp32/fp16, target fp32,
+    val_mask [B,1,H,W] bool.  Returns (loss 0-d fp32 device tensor, 0 for an empty mask; latent_mask [B,h,w] uint8;
+    workspace fp64 [2] = (sum, count)) — the last two feed masked_latent_mse_bwd."""
+    _need_cuda(pred, target, val_mask)
+    B, C, H, W, h, w = latent_mask_shape(val_mask, pred)
+    assert pred.dtype in (F16, F32) and pred.is_contiguous() and target.dtype == F32 and target.is_contiguous()
+    assert target.shape == pred.shape
+    vm = val_mask if val_mask.dtype in (torch.bool, torch.uint8) else val_mask.to(torch.bool)
+    vm = vm.contiguous()
+    lm = torch.empty((B, h, w), dtype=torch.uint8, device=pred.device)
+    ws = torch.zeros(2, dtype=torch.float64, device=pred.device)
+    out = torch.empty(1, dtype=F32, device=pred.device)
+    _ck(_lib.load().b200_masked_latent_mse(_p(pred), int(pred.dtype == F16), _p(target), _p(vm), B, C, H, W, h, w,
+                                           _p(lm), _p(ws), _p(out), _stream()), "b200_masked_latent_mse")
+    return out[0], lm, ws
+
+
+@_timed("loss")
+def masked_latent_mse_bwd(pred, target, latent_mask, workspace, grad_out):
+    """d masked_latent_mse / d pred * grad_out (0-d fp32 device tensor) -> pred's dtype and shape."""
+    _need_cuda(pred, target, latent_mask, workspace, grad_out)
+    assert pred.is_contiguous() and target.is_contiguous() and latent_mask.is_contiguous()
+    n, C, h, w = pred.shape
+    go = grad_out.detach().to(F32).reshape(1).contiguous()
+    grad = torch.empty_like(pred)
+    _ck(_lib.load().b200_masked_latent_mse_bwd(_p(pred), int(pred.dtype == F16), _p(target), _p(latent_mask),
+                                               _p(workspace), _p(go), n // 2, C, h * w, _p(grad), _stream()),
+        "b200_masked_latent_mse_bwd")
+    return grad
+
+
+@_timed("optim")
+def ema_update(ema, param, one_minus_decay):
+    """ema <- ema - one_minus_decay * (ema - param) over flat fp32 buffers, in place (diffusers EMAModel.step);
+    `one_minus_decay` is a host float, so there is no sync."""
+    _need_cuda(ema, param)
+    assert ema.dtype == F32 and param.dtype == F32 and ema.is_contiguous() and param.is_contiguous()
+    assert ema.numel() == param.numel()
+    _ck(_lib.load().b200_ema_update(_p(ema), _p(param), ema.numel(), float(one_minus_decay), _stream()),
+        "b200_ema_update")

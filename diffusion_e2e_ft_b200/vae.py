@@ -304,8 +304,9 @@ class B200AutoencoderKL(PretrainedMixin, nn.Module):
         s = 1.0 / self.config["scaling_factor"]
         if torch.is_grad_enabled() and model_out.requires_grad:
             from . import autograd_blocks as ab
-            if noisy is not None and c_noisy != 0.0:
-                raise NotImplementedError("differentiable decode supports the x_t = 0 recipe (noise_type zeros) only")
-            return self.decoder(ab.pointwise(self.post_quant_conv, model_out, c_out * s))
+            if noisy is None or c_noisy == 0.0:
+                return self.decoder(ab.pointwise(self.post_quant_conv, model_out, c_out * s))
+            # noisy-start E2E fine-tuning: c_noisy * x_t is a constant addend, so the backward is unchanged
+            return self.decoder(ab.pointwise(self.post_quant_conv, model_out, c_out * s, noisy, c_noisy * s))
         z = self.post_quant_conv(model_out, scale_in=c_out * s, x2=noisy, scale_in2=c_noisy * s)
         return self.decoder(z)

@@ -362,6 +362,34 @@ int b200_colorize_depth(const float* x, long long n, const unsigned char* table,
                         void* stream);
 int b200_colorize_normals(const float* x, long long HW, unsigned char* out, void* stream);
 
+/* Diffusion-objective training and the EMA of the UNet weights (ABI 10).
+ * b200_diffusion_inputs: DDPMScheduler.add_noise + get_velocity + the UNet-input concatenation of
+ *   GeoWizard/geowizard/training/train_depth_normal.py:666-705 (the default, non-`--e2e_ft` branch) in one pass.
+ *   rgb_latents [B][C][HW], x0 / noise [2B][C][HW] (depth half, then normal half; noise NULL = zeros), timesteps int64
+ *   [2B] and alphas_cumprod fp32 [T] on the device (0 <= t < T, checked by the caller), all fp32.  With a = ac[t[n]]:
+ *     unet_in [2B][2C][HW] = [rgb[n mod B] | sqrt(a) x0 + sqrt(1 - a) eps],
+ *     target  [2B][C][HW]  = eps (B200_PRED_EPSILON) or sqrt(a) eps - sqrt(1 - a) x0 (B200_PRED_V),
+ *   each product and sum rounded on its own: bit-identical to torch's fp32 evaluation of diffusers' expressions.
+ * b200_masked_latent_mse: F.mse_loss(pred[latent_mask], target[latent_mask]) of :607-609,712-714 with
+ *   latent_mask = ~max_pool2d(~val_mask, 8, 8) repeated over the 2 halves and C channels.  pred [2B][C][h][w]
+ *   (pred_f16 ? fp16 : fp32), target fp32, val_mask [B][H][W] bytes with h = H / 8, w = W / 8.  Writes latent_mask
+ *   [B][h][w] bytes (for the backward), workspace (2 zeroed doubles: fp64 sum of squares, exact count) and out[0] =
+ *   sum / count, 0 for an empty mask.  No host sync.
+ * b200_masked_latent_mse_bwd: grad = grad_out[0] * 2 (pred - target) / count on the latent mask, 0 elsewhere, in
+ *   pred's dtype and layout; latent_mask and workspace are the forward's.
+ * b200_ema_update: diffusers EMAModel.step (train_depth_normal.py:351-353,785-786) over flat fp32 buffers:
+ *   ema <- ema - one_minus_decay * (ema - param), each operation rounded on its own; 16-byte aligned buffers. */
+int b200_diffusion_inputs(const float* rgb_latents, const float* x0, const float* noise, const long long* timesteps,
+                          const float* alphas_cumprod, int B, int C, long long HW, int prediction_type, float* unet_in,
+                          float* target, void* stream);
+int b200_masked_latent_mse(const void* pred, int pred_f16, const float* target, const unsigned char* val_mask, int B,
+                           int C, int H, int W, int h, int w, unsigned char* latent_mask, double* workspace, float* out,
+                           void* stream);
+int b200_masked_latent_mse_bwd(const void* pred, int pred_f16, const float* target, const unsigned char* latent_mask,
+                               const double* workspace, const float* grad_out, int B, int C, long long hw, void* grad,
+                               void* stream);
+int b200_ema_update(float* ema, const float* param, long long n, float one_minus_decay, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
