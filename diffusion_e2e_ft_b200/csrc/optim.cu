@@ -88,31 +88,83 @@ __global__ void optim_prepare_kernel(const double* __restrict__ gnorm_sq, float*
   state[1] = tracker;
 }
 
+// Per-group learning rate / weight decay (torch.optim.AdamW parameter groups, ABI 11): the flat buffer is cut into
+// RUNS, contiguous ranges [run_start[r], run_start[r+1]) each belonging to one group; run_start is increasing, starts
+// at 0 and every start is a multiple of 4 (each parameter view starts 16-byte aligned), so a float4 never straddles
+// two groups.  The run table (device) is staged in shared memory and a float4's run found by binary search; the
+// per-group (lr, weight_decay) pairs travel as launch arguments.  run_start == nullptr: one run, group 0, taking
+// the one-group loops of the kernel before ABI 11 unchanged.
+struct AdamwGroupHP {
+  float lr[B200_ADAMW_MAX_GROUPS];
+  float wd[B200_ADAMW_MAX_GROUPS];
+};
+
 __global__ void adamw_state_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                   float* __restrict__ v, long long n, float lr, float beta1, float beta2, float eps,
-                                   float wd, const float* __restrict__ state) {
-  if (state[4] != 0.f) return;                                   // skipped step: nothing is touched
+                                   float* __restrict__ v, long long n, const long long* __restrict__ run_start,
+                                   const int* __restrict__ run_group, int n_runs, AdamwGroupHP hp, int n_groups,
+                                   float beta1, float beta2, float eps, const float* __restrict__ state) {
+  __shared__ long long s_start[B200_ADAMW_MAX_RUNS];
+  __shared__ int s_group[B200_ADAMW_MAX_RUNS];
+  __shared__ float s_decay[B200_ADAMW_MAX_GROUPS], s_step[B200_ADAMW_MAX_GROUPS];
+  if (state[4] != 0.f) return;                                   // skipped step: nothing is touched (block-uniform)
   const float clip = state[5], bc1 = state[6], rbc2 = rsqrtf(state[7]);
   const long long n4 = n / 4;
   float4* p4 = reinterpret_cast<float4*>(p);
   const float4* g4 = reinterpret_cast<const float4*>(g);
   float4* m4 = reinterpret_cast<float4*>(m);
   float4* v4 = reinterpret_cast<float4*>(v);
-  const float decay = 1.0f - lr * wd, step_size = lr / bc1;
-  auto upd = [&](float& pi, float gi, float& mi, float& vi) {
+  auto upd = [&](float& pi, float gi, float& mi, float& vi, float decay, float step_size) {
     gi *= clip;
     mi = beta1 * mi + (1.0f - beta1) * gi;
     vi = beta2 * vi + (1.0f - beta2) * gi * gi;
     pi = pi * decay - step_size * (mi / (sqrtf(vi) * rbc2 + eps));
   };
+  if (run_start == nullptr) {
+    // one group: the loops of the kernel before ABI 11, with decay / step_size held in registers, so the compiled
+    // update (and its rounding) is the one b200_adamw_step_state always had
+    const float decay = 1.0f - hp.lr[0] * hp.wd[0], step_size = hp.lr[0] / bc1;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+      float4 pp = p4[i], mm = m4[i], vv = v4[i];
+      const float4 gg = g4[i];
+      upd(pp.x, gg.x, mm.x, vv.x, decay, step_size); upd(pp.y, gg.y, mm.y, vv.y, decay, step_size);
+      upd(pp.z, gg.z, mm.z, vv.z, decay, step_size); upd(pp.w, gg.w, mm.w, vv.w, decay, step_size);
+      p4[i] = pp; m4[i] = mm; v4[i] = vv;
+    }
+    for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+      upd(p[i], g[i], m[i], v[i], decay, step_size);
+    return;
+  }
+  for (int r = threadIdx.x; r < n_runs; r += blockDim.x) {
+    s_start[r] = run_start[r];
+    s_group[r] = min(max(run_group[r], 0), n_groups - 1);
+  }
+  if ((int)threadIdx.x < n_groups) {
+    const float lr = hp.lr[threadIdx.x], wd = hp.wd[threadIdx.x];
+    s_decay[threadIdx.x] = 1.0f - lr * wd;
+    s_step[threadIdx.x] = lr / bc1;
+  }
+  __syncthreads();
+  auto group_of = [&](long long e) {                             // the last run starting at or before element e
+    int lo = 0, hi = n_runs - 1;
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (s_start[mid] <= e) lo = mid; else hi = mid - 1;
+    }
+    return s_group[lo];
+  };
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const int k = group_of(4 * i);
+    const float decay = s_decay[k], step_size = s_step[k];
     float4 pp = p4[i], mm = m4[i], vv = v4[i];
     const float4 gg = g4[i];
-    upd(pp.x, gg.x, mm.x, vv.x); upd(pp.y, gg.y, mm.y, vv.y); upd(pp.z, gg.z, mm.z, vv.z); upd(pp.w, gg.w, mm.w, vv.w);
+    upd(pp.x, gg.x, mm.x, vv.x, decay, step_size); upd(pp.y, gg.y, mm.y, vv.y, decay, step_size);
+    upd(pp.z, gg.z, mm.z, vv.z, decay, step_size); upd(pp.w, gg.w, mm.w, vv.w, decay, step_size);
     p4[i] = pp; m4[i] = mm; v4[i] = vv;
   }
-  for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    upd(p[i], g[i], m[i], v[i]);
+  for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const int k = group_of(i);
+    upd(p[i], g[i], m[i], v[i], s_decay[k], s_step[k]);
+  }
 }
 
 // diffusers EMAModel.step: s_param.sub_(one_minus_decay * (s_param - param)), each operation rounded on its own.
@@ -147,24 +199,43 @@ extern "C" int b200_ema_update(float* ema, const float* param, long long n, floa
   return 0;
 }
 
-extern "C" int b200_adamw_step_state(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
-                                     float lr, float beta1, float beta2, float eps, float weight_decay,
-                                     const double* grad_norm_sq, float max_grad_norm, float inv_world, float* state,
-                                     int dynamic_scale, float growth_interval, float min_scale, float max_scale,
-                                     void* stream) {
+extern "C" int b200_adamw_step_state_groups(float* param, const float* grad, float* exp_avg, float* exp_avg_sq,
+                                            long long n, const long long* run_start, const int* run_group, int n_runs,
+                                            const float* group_lr, const float* group_wd, int n_groups, float beta1,
+                                            float beta2, float eps, const double* grad_norm_sq, float max_grad_norm,
+                                            float inv_world, float* state, int dynamic_scale, float growth_interval,
+                                            float min_scale, float max_scale, void* stream) {
   B200_CHECK_ARG(param && grad && exp_avg && exp_avg_sq && grad_norm_sq && state && n > 0 && inv_world > 0.f,
-                 "b200_adamw_step_state: bad arguments");
+                 "b200_adamw_step_state_groups: bad arguments");
   B200_CHECK_ARG((((uintptr_t)param | (uintptr_t)grad | (uintptr_t)exp_avg | (uintptr_t)exp_avg_sq) & 15) == 0,
-                 "b200_adamw_step_state: buffers must be 16-byte aligned");
+                 "b200_adamw_step_state_groups: buffers must be 16-byte aligned");
+  B200_CHECK_ARG(group_lr && group_wd && n_groups >= 1 && n_groups <= B200_ADAMW_MAX_GROUPS,
+                 "b200_adamw_step_state_groups: 1..%d groups with host lr / weight_decay arrays", B200_ADAMW_MAX_GROUPS);
+  B200_CHECK_ARG(n_runs >= 1 && n_runs <= B200_ADAMW_MAX_RUNS && (n_runs == 1 || (run_start && run_group)),
+                 "b200_adamw_step_state_groups: 1..%d runs (device run_start / run_group needed for more than one)",
+                 B200_ADAMW_MAX_RUNS);
+  AdamwGroupHP hp{};
+  for (int k = 0; k < n_groups; ++k) { hp.lr[k] = group_lr[k]; hp.wd[k] = group_wd[k]; }
   cudaStream_t st = (cudaStream_t)stream;
   optim_prepare_kernel<<<1, 1, 0, st>>>(grad_norm_sq, state, max_grad_norm, inv_world, beta1, beta2, dynamic_scale,
                                         growth_interval, min_scale, max_scale);
   long long g = (n / 4 + 255) / 256;
   long long cap = (long long)sm_count() * 8;
-  adamw_state_kernel<<<(unsigned)(g < 1 ? 1 : (g > cap ? cap : g)), 256, 0, st>>>(param, grad, exp_avg, exp_avg_sq, n, lr, beta1,
-                                                                                  beta2, eps, weight_decay, state);
+  adamw_state_kernel<<<(unsigned)(g < 1 ? 1 : (g > cap ? cap : g)), 256, 0, st>>>(
+      param, grad, exp_avg, exp_avg_sq, n, n_runs == 1 ? nullptr : run_start, run_group, n_runs, hp, n_groups, beta1,
+      beta2, eps, state);
   B200_CHECK_LAUNCH("adamw_state_kernel");
   return 0;
+}
+
+extern "C" int b200_adamw_step_state(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
+                                     float lr, float beta1, float beta2, float eps, float weight_decay,
+                                     const double* grad_norm_sq, float max_grad_norm, float inv_world, float* state,
+                                     int dynamic_scale, float growth_interval, float min_scale, float max_scale,
+                                     void* stream) {
+  return b200_adamw_step_state_groups(param, grad, exp_avg, exp_avg_sq, n, nullptr, nullptr, 1, &lr, &weight_decay, 1,
+                                      beta1, beta2, eps, grad_norm_sq, max_grad_norm, inv_world, state, dynamic_scale,
+                                      growth_interval, min_scale, max_scale, stream);
 }
 
 extern "C" int b200_sumsq(const float* x, long long n, double* out, void* stream) {

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 10        # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 11        # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -75,6 +75,8 @@ _SIGS = {
                                        c_float, c_float, _P]),
     "b200_adamw_step_state": (c_int, [_P, _P, _P, _P, _LL, c_float, c_float, c_float, c_float, c_float, _P, c_float,
                                       c_float, _P, c_int, c_float, c_float, c_float, _P]),
+    "b200_adamw_step_state_groups": (c_int, [_P, _P, _P, _P, _LL, _P, _P, c_int, _P, _P, c_int, c_float, c_float,
+                                             c_float, _P, c_float, c_float, _P, c_int, c_float, c_float, c_float, _P]),
     "b200_upsample_nearest_bwd": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, _P]),
     "b200_ensemble_normals": (c_int, [_P, c_int, _LL, _P, _P, _P, _P]),
     "b200_ensemble_depths_objective": (c_int, [_P, _P, _P, c_int, _LL, c_int, _P, _P, _P]),

@@ -5,7 +5,7 @@ launched on `torch.cuda.current_stream()`.  Nothing in this module computes with
 exceptions that are O(channels) in size: dtype conversions of masks / loss inputs at the API boundary and the
 final [NB, C, 2] -> [C, 2] fold of the GroupNorm-backward partial sums.
 """
-from ctypes import c_int, c_void_p
+from ctypes import c_float, c_int, c_void_p
 
 import torch
 
@@ -571,6 +571,50 @@ def adamw_step_state(param, grad, exp_avg, exp_avg_sq, state, grad_norm_sq_t, lr
                                           _p(grad_norm_sq_t), float(max_grad_norm), float(inv_world), _p(state),
                                           int(dynamic_scale), float(growth_interval), float(min_scale), float(max_scale),
                                           _stream()), "b200_adamw_step_state")
+
+
+ADAMW_MAX_GROUPS, ADAMW_MAX_RUNS = 16, 1024            # B200_ADAMW_MAX_GROUPS / B200_ADAMW_MAX_RUNS
+
+
+def adamw_run_table(starts, groups, n, n_groups, device):
+    """Check a run table on the host and put it on the device: run r covers [starts[r], starts[r+1]) of a flat
+    buffer of n elements and belongs to group groups[r].  Returns (run_start int64, run_group int32) device tensors."""
+    starts, groups = [int(s) for s in starts], [int(k) for k in groups]
+    if not 1 <= len(starts) <= ADAMW_MAX_RUNS or len(groups) != len(starts):
+        raise ValueError(f"a run table has 1..{ADAMW_MAX_RUNS} runs with one group each, got {len(starts)} starts and "
+                         f"{len(groups)} groups")
+    if not 1 <= n_groups <= ADAMW_MAX_GROUPS:
+        raise ValueError(f"1..{ADAMW_MAX_GROUPS} parameter groups, got {n_groups}")
+    if starts[0] != 0 or any(b <= a for a, b in zip(starts, starts[1:])) or starts[-1] >= n or any(s % 4 for s in starts):
+        raise ValueError("run starts must begin at 0, increase, stay below the buffer size and be multiples of 4")
+    if any(not 0 <= k < n_groups for k in groups):
+        raise ValueError(f"run groups must lie in [0, {n_groups})")
+    return (torch.tensor(starts, dtype=torch.int64).to(device), torch.tensor(groups, dtype=torch.int32).to(device))
+
+
+@_timed("optim")
+def adamw_step_state_groups(param, grad, exp_avg, exp_avg_sq, state, grad_norm_sq_t, run_start, run_group, group_lr,
+                            group_wd, betas=(0.9, 0.999), eps=1e-8, max_grad_norm=0.0, inv_world=1.0, dynamic_scale=True,
+                            growth_interval=2000, min_scale=1.0, max_scale=65536.0):
+    """`adamw_step_state` with per-group learning rate and weight decay (torch.optim.AdamW parameter groups,
+    train_depth_normal.py:428-444): `run_start` / `run_group` from `adamw_run_table`, `group_lr` / `group_wd` one
+    float per group.  One skip decision, loss scale and bias correction for all groups, as in torch."""
+    _need_cuda(param, grad, exp_avg, exp_avg_sq, state, grad_norm_sq_t, run_start, run_group)
+    for t in (param, grad, exp_avg, exp_avg_sq):
+        assert t.dtype == F32 and t.is_contiguous() and t.numel() == param.numel()
+    assert state.dtype == F32 and state.numel() == 8 and state.is_contiguous()
+    assert run_start.dtype == torch.int64 and run_group.dtype == torch.int32 and run_start.is_contiguous() \
+        and run_group.is_contiguous() and run_start.numel() == run_group.numel()
+    n_groups = len(group_lr)
+    if len(group_wd) != n_groups or not 1 <= n_groups <= ADAMW_MAX_GROUPS:
+        raise ValueError(f"one lr and one weight_decay per group, 1..{ADAMW_MAX_GROUPS} groups")
+    lr_h, wd_h = (c_float * n_groups)(*map(float, group_lr)), (c_float * n_groups)(*map(float, group_wd))
+    _ck(_lib.load().b200_adamw_step_state_groups(_p(param), _p(grad), _p(exp_avg), _p(exp_avg_sq), param.numel(),
+                                                 _p(run_start), _p(run_group), run_start.numel(), lr_h, wd_h, n_groups,
+                                                 float(betas[0]), float(betas[1]), float(eps), _p(grad_norm_sq_t),
+                                                 float(max_grad_norm), float(inv_world), _p(state), int(dynamic_scale),
+                                                 float(growth_interval), float(min_scale), float(max_scale), _stream()),
+        "b200_adamw_step_state_groups")
 
 
 @_timed("cast")

@@ -10,6 +10,7 @@ output dataclasses — and route the arithmetic through B200UNet2DConditionModel
   DDIMScheduler (eta = 0, step on the b200_ddim_step kernel) <- diffusers DDIMScheduler as used at
                                    marigold_pipeline.py:401-402,457-465 and geowizard_pipeline.py:261,326-334
 """
+import gc
 import json
 import math
 import os
@@ -230,8 +231,18 @@ class PipelineBase:
             torch.cuda.synchronize()
             before = (ops.STATS.launches, dict(ops.STATS.flops), dict(ops.STATS.count))
             g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                out = fn(*static_xs)
+            # No cyclic garbage collection while capturing: a collection can free an unreachable pipeline (e.g. one
+            # whose methods were wrapped in closures) together with its captured graphs, and destroying a graph is
+            # not permitted while a stream captures, which invalidates this capture.  torch no longer collects
+            # before a capture, so the collector stays off for its duration and runs afterwards as usual.
+            gc_on = gc.isenabled()
+            gc.disable()
+            try:
+                with torch.cuda.graph(g):
+                    out = fn(*static_xs)
+            finally:
+                if gc_on:
+                    gc.enable()
             delta = dict(launches=ops.STATS.launches - before[0],
                          flops={k: ops.STATS.flops[k] - before[1][k] for k in before[1]},
                          count={k: ops.STATS.count[k] - before[2][k] for k in before[2]})

@@ -262,6 +262,85 @@ def ema_config(step, decay=EMA_DECAY):
                 inv_gamma=1.0, power=2 / 3)
 
 
+ADAM_BETAS, ADAM_EPS = (0.9, 0.999), 1e-8        # train.py:346-353 / train_depth_normal.py:437-444 defaults
+
+
+class IterExponential:
+    """Marigold's iteration-wise LR factor (training/util/lr_scheduler.py, used by both recipes through LambdaLR):
+    linear warm-up 0 -> 1 over `warmup_steps`, then exp(t / (total - warmup) * log(final_ratio)) in float64, held at
+    `final_ratio` from `total_iter_length` on.  The attribute names are the reference's, so LambdaLR.state_dict()
+    stores the same `lr_lambdas` entry and either side loads the other's scheduler.bin."""
+
+    def __init__(self, total_iter_length, final_ratio, warmup_steps=0):
+        self.total_length = total_iter_length
+        self.effective_length = total_iter_length - warmup_steps
+        self.final_ratio = final_ratio
+        self.warmup_steps = warmup_steps
+
+    def __call__(self, n_iter):
+        import numpy as np
+        if n_iter < self.warmup_steps:
+            return 1.0 * n_iter / self.warmup_steps
+        if n_iter >= self.total_length:
+            return self.final_ratio
+        return np.exp((n_iter - self.warmup_steps) / self.effective_length * np.log(self.final_ratio))
+
+
+class ConstantLR:
+    """GeoWizard's `--lr_scheduler constant` (diffusers get_scheduler("constant")): factor 1 on every step; the
+    warm-up argument is ignored, as diffusers ignores it for this choice."""
+
+    def __init__(self, *unused, **unused_kw):
+        pass
+
+    def __call__(self, n_iter):
+        return 1.0
+
+
+def geowizard_param_groups(class_embedding_lr_mult=10.0):
+    """The two AdamW parameter groups of train_depth_normal.py:428-444: every parameter without `class_embedding` in
+    its name at the base learning rate, then the `class_embedding.*` parameters at base * class_embedding_lr_mult
+    (the script's default is 10).  Pass as FlatTrainer(..., param_groups=geowizard_param_groups())."""
+    return [dict(name="params", select=lambda n: "class_embedding" not in n, lr_mult=1.0),
+            dict(name="params_class_embedding", select=lambda n: "class_embedding" in n,
+                 lr_mult=float(class_embedding_lr_mult))]
+
+
+_CHECKPOINT_RE = r"checkpoint-(\d+)$"
+
+
+def _checkpoints(output_dir):
+    import os
+    import re
+    if not os.path.isdir(output_dir):
+        return []
+    found = [(int(m.group(1)), d) for d in os.listdir(output_dir) if (m := re.match(_CHECKPOINT_RE, d))]
+    return [d for _, d in sorted(found)]
+
+
+def latest_checkpoint(output_dir):
+    """`--resume_from_checkpoint latest` (train.py:416-425): the path of the `checkpoint-N` folder in `output_dir`
+    with the largest N (numeric order, so checkpoint-1000 follows checkpoint-900), or None when there is none."""
+    import os
+    cps = _checkpoints(output_dir)
+    return os.path.join(output_dir, cps[-1]) if cps else None
+
+
+def prune_checkpoints(output_dir, total_limit):
+    """`--checkpoints_total_limit` (train.py:581-596), called BEFORE a save: delete the oldest `checkpoint-N` folders
+    so that at most total_limit - 1 remain, making room for the one about to be written.  Returns the removed paths;
+    total_limit None keeps everything."""
+    import os
+    import shutil
+    if total_limit is None:
+        return []
+    cps = _checkpoints(output_dir)
+    removed = [os.path.join(output_dir, d) for d in cps[:max(0, len(cps) - int(total_limit) + 1)]]
+    for d in removed:
+        shutil.rmtree(d)
+    return removed
+
+
 class FlatTrainer:
     """The optimizer side of training/train.py:346-353,560-568 for one module (the UNet): all trainable parameters
     and their gradients are re-homed as views of two flat fp32 buffers, so `backward()` accumulates straight into
@@ -291,17 +370,38 @@ class FlatTrainer:
     Mixed precision: backward GEMM operands are fp16, so the loss is multiplied by a loss scale held ON THE DEVICE
     (`state[0]`); the fused optimizer kernel skips the step and halves the scale when the gradient norm is non-finite,
     doubles it after `growth_interval` good steps, and also skips when the gradient is exactly zero (all masks empty:
-    train.py:503,546-551) — all without a host sync.  `skipped_steps()` / `loss_scale()` read the state back."""
+    train.py:503,546-551) — all without a host sync.  `skipped_steps()` / `loss_scale()` read the state back.
+
+    Parameter groups (`param_groups`, torch.optim.AdamW's groups): None is one group over every trainable parameter
+    (train.py:346-353).  Otherwise an ordered list of dicts `dict(name=..., select=lambda param_name: bool,
+    lr_mult=1.0, weight_decay=None)`; each parameter joins the first group that selects it, trains at lr * lr_mult
+    with the group's weight decay (None: the trainer's), and every parameter must land in a group.
+    `geowizard_param_groups()` gives train_depth_normal.py:428-444.  The flat layout is not reordered: the fused
+    kernel finds each element's group from a table of contiguous runs.  Group order, then named_parameters order
+    within a group, numbers the parameters in the saved optimizer state, as torch numbers them.
+
+    LR schedule (`lr_schedule`, e.g. `IterExponential(20000 * N, 0.01, 100 * N)` built with the reference's own
+    arguments, or `ConstantLR()`): optimizer step k (0-based, every step() call counted) runs at
+    lr_g = lr * lr_mult_g * lr_schedule(k * N), N = `num_processes` (default: the world size).  That is what LambdaLR
+    gives under accelerate, whose scheduler wrapper steps it N times per optimizer step — INCLUDING lr = 0 on step 0
+    with a warm-up, because LambdaLR applies lambda(0) before the first step.  Steps the device skips (zero or
+    non-finite gradient) still advance the schedule, as the reference's scheduler steps after an AdamW step that
+    updated nothing; so the rates are known on the host without a sync.  `get_last_lr()` is the rates of the next step.
+
+    Checkpoints: `save_state(dir)` / `load_state(dir)` write and read accelerate's `checkpoint-N` folder (unet/,
+    unet_ema/, optimizer.bin, scheduler.bin, random_states_{rank}.pkl) plus the engine's flat_trainer.pt;
+    `latest_checkpoint` and `prune_checkpoints` are the scripts' folder logic."""
 
     LATE_GRAD_KEYS = ("time_emb_proj", "time_embedding", "class_embedding")
 
     def __init__(self, module, lr=3e-5, weight_decay=1e-2, max_grad_norm=1.0, accumulation_steps=1, group=None,
                  loss_scale=LOSS_SCALE, bucket_mb=256, dynamic_loss_scale=True, growth_interval=2000, overlap=False,
-                 use_ema=False):
+                 use_ema=False, param_groups=None, lr_schedule=None, num_processes=None):
         import torch.distributed as dist
         named = [(n, p) for n, p in module.named_parameters() if p.requires_grad]
         if not named:
             raise ValueError("no trainable parameters")
+        self._group_def = self._resolve_groups(named, param_groups, weight_decay)
         late = [(n, p) for n, p in named if any(k in n for k in self.LATE_GRAD_KEYS)]
         rest = [(n, p) for n, p in named if not any(k in n for k in self.LATE_GRAD_KEYS)]
         ps = [p for _, p in late] + [p for _, p in rest]          # flat order == reverse gradient-ready order
@@ -336,6 +436,18 @@ class FlatTrainer:
                     self._buckets.append(dict(lo=start, hi=off, n=count))
                     start, count = off, 0
         self.params, self.step_count = ps, 0
+        # contiguous runs of one group along the flat layout, for the fused kernel
+        group_of = {n: k for k, g in enumerate(self._group_def) for n in g["params"]}
+        runs = []
+        for name, off, _ in self._layout:
+            if not runs or runs[-1][1] != group_of[name]:
+                runs.append((off, group_of[name]))
+        self._runs = runs
+        self._run_table = None if len(runs) == 1 else ops.adamw_run_table(
+            [r[0] for r in runs], [r[1] for r in runs], total, len(self._group_def), dev)
+        self.lr_schedule = lr_schedule
+        self.num_processes = int(num_processes) if num_processes is not None else self.world
+        self._init_loss_scale = float(loss_scale)
         self.lr, self.weight_decay, self.max_grad_norm = lr, weight_decay, max_grad_norm
         self.accumulation_steps, self.group = max(1, int(accumulation_steps)), group
         self.dynamic_loss_scale, self.growth_interval, self.overlap = dynamic_loss_scale, growth_interval, overlap
@@ -378,9 +490,45 @@ class FlatTrainer:
         self._micro += 1
         (loss * (self.state[0] / self.accumulation_steps)).backward()
 
+    @staticmethod
+    def _resolve_groups(named, param_groups, weight_decay):
+        if param_groups is None:
+            param_groups = [dict(name="params", select=None)]
+        if not 1 <= len(param_groups) <= ops.ADAMW_MAX_GROUPS:
+            raise ValueError(f"1..{ops.ADAMW_MAX_GROUPS} parameter groups, got {len(param_groups)}")
+        groups = []
+        for k, g in enumerate(param_groups):
+            wd = g.get("weight_decay")
+            groups.append(dict(name=str(g.get("name", f"group_{k}")), lr_mult=float(g.get("lr_mult", 1.0)),
+                               weight_decay=float(weight_decay if wd is None else wd), params=[]))
+        for n, _ in named:
+            k = next((k for k, g in enumerate(param_groups) if g.get("select") is None or g["select"](n)), None)
+            if k is None:
+                raise ValueError(f"parameter {n} is in no parameter group")
+            groups[k]["params"].append(n)
+        return groups
+
+    def _lrs(self, k, lr=None):
+        """Per-group learning rates of optimizer step k (0-based)."""
+        if self.lr_schedule is not None:
+            f = self.lr_schedule(k * self.num_processes)
+            return [float(self.lr * g["lr_mult"] * f) for g in self._group_def]
+        base = self.lr if lr is None else lr
+        return [base * g["lr_mult"] for g in self._group_def]
+
+    def get_last_lr(self):
+        """The per-group learning rates the next step() will use (LambdaLR.get_last_lr(), logged at train.py:575 /
+        train_depth_normal.py:791)."""
+        return self._lrs(self.step_count)
+
+    def _check_lr_arg(self, lr):
+        if lr is not None and self.lr_schedule is not None:
+            raise ValueError("lr= and lr_schedule are exclusive: the schedule sets every step's learning rate")
+
     def micro_step(self, loss, lr=None):
         """backward(); on the last micro-step of the accumulation window also step().  Returns True when it stepped
         (`accelerator.sync_gradients` of train.py:563-570)."""
+        self._check_lr_arg(lr)
         self.backward(loss)
         if self._micro % self.accumulation_steps == 0:
             self.step(lr)
@@ -388,9 +536,11 @@ class FlatTrainer:
         return False
 
     def step(self, lr=None):
+        self._check_lr_arg(lr)
         if self._micro % self.accumulation_steps != 0 or not self._synced:
             raise RuntimeError(f"FlatTrainer.step inside an accumulation window ({self._micro % self.accumulation_steps} of "
                                f"{self.accumulation_steps} micro-steps) or after backward(sync=False): gradients are not reduced")
+        lrs, wds = self._lrs(self.step_count, lr), [g["weight_decay"] for g in self._group_def]
         self.step_count += 1
         if self.world > 1:
             for b in range(len(self._buckets)):                    # parameters without a gradient this step / overlap off
@@ -401,10 +551,17 @@ class FlatTrainer:
             self._handles = {}
         from .modules import bump_weights_epoch
         nsq = ops.grad_norm_sq(self.flat_grad)
-        ops.adamw_step_state(self.flat_param, self.flat_grad, self.exp_avg, self.exp_avg_sq, self.state, nsq,
-                             lr=self.lr if lr is None else lr, weight_decay=self.weight_decay,
-                             max_grad_norm=self.max_grad_norm, inv_world=1.0 / self.world,
-                             dynamic_scale=self.dynamic_loss_scale, growth_interval=self.growth_interval)
+        if self._run_table is None:                                # one run: the whole buffer is one group
+            k = self._runs[0][1]
+            ops.adamw_step_state(self.flat_param, self.flat_grad, self.exp_avg, self.exp_avg_sq, self.state, nsq,
+                                 lr=lrs[k], weight_decay=wds[k], max_grad_norm=self.max_grad_norm,
+                                 inv_world=1.0 / self.world, dynamic_scale=self.dynamic_loss_scale,
+                                 growth_interval=self.growth_interval)
+        else:
+            ops.adamw_step_state_groups(self.flat_param, self.flat_grad, self.exp_avg, self.exp_avg_sq, self.state, nsq,
+                                        *self._run_table, lrs, wds, max_grad_norm=self.max_grad_norm,
+                                        inv_world=1.0 / self.world, dynamic_scale=self.dynamic_loss_scale,
+                                        growth_interval=self.growth_interval)
         bump_weights_epoch()
         self.flat_grad.zero_()
         if self.ema is not None:
@@ -453,20 +610,197 @@ class FlatTrainer:
     def load_ema(self, directory):
         """EMAModel.from_pretrained + load_state_dict: the EMA weights and step count written by save_ema (or by
         diffusers' EMAModel.save_pretrained) into the EMA buffer."""
+        self._need_ema()
+        step, flat = self._read_ema(directory)
+        self.ema.copy_(flat)
+        self.ema_steps = step
+
+    def _read_ema(self, directory):
         import json
         import os
-        from .checkpoint import CONFIG_NAME, load_weights
-        self._need_ema()
+        from .checkpoint import CONFIG_NAME
         with open(os.path.join(directory, CONFIG_NAME)) as f:
             step = int(json.load(f).get("optimization_step", 0))
+        return step, self._flat_from(self._load_checked(directory, "EMA weight"))
+
+    def _load_checked(self, directory, what):
+        """The weights of a diffusers folder, checked against the trainer's parameter names and shapes."""
+        from .checkpoint import load_weights
         sd = load_weights(directory)
+        for name, _, shape in self._layout:
+            if name not in sd or tuple(sd[name].shape) != shape:
+                raise ValueError(f"{directory}: no {what} {name} of shape {list(shape)}")
+        return sd
+
+    def _flat_from(self, per_param):
+        """A host flat buffer in the trainer's layout from {name: tensor} (padding zero)."""
+        flat = torch.zeros(self.flat_param.numel(), dtype=torch.float32)
+        for name, off, shape in self._layout:
+            flat[off:off + math.prod(shape)].copy_(per_param[name].reshape(-1))
+        return flat
+
+    # ---- save / resume of the whole training state (accelerator.save_state / load_state, train.py:416-438,578-598,
+    # train_depth_normal.py:376-404,540-563,811-831)
+    def _torch_order(self):
+        """(group, diffusers name) per torch parameter index: group order, then named_parameters order."""
+        return [(k, n) for k, g in enumerate(self._group_def) for n in g["params"]]
+
+    def _check_boundary(self, what):
+        if self._micro % self.accumulation_steps != 0 or self._handles:
+            raise RuntimeError(f"FlatTrainer.{what} inside an accumulation window ({self._micro % self.accumulation_steps} "
+                               f"of {self.accumulation_steps} micro-steps): call it after the step")
+
+    def _torch_param_groups(self):
+        """torch.optim.AdamW param_groups as the reference's optimizer holds them after `step_count` scheduler steps:
+        torch's own defaults for this version, plus lr / initial_lr / betas / eps / weight_decay and the indices."""
+        template = torch.optim.AdamW([torch.zeros(1)], lr=1.0, betas=ADAM_BETAS, eps=ADAM_EPS,
+                                     weight_decay=0.0).state_dict()["param_groups"][0]
+        lrs, out, idx = self.get_last_lr(), [], 0
+        for k, g in enumerate(self._group_def):
+            d = dict(template)
+            d.update(lr=lrs[k], initial_lr=self.lr * g["lr_mult"], betas=ADAM_BETAS, eps=ADAM_EPS,
+                     weight_decay=g["weight_decay"], params=list(range(idx, idx + len(g["params"]))))
+            idx += len(g["params"])
+            out.append(d)
+        return out
+
+    def _scheduler_state_dict(self):
+        """LambdaLR.state_dict() of the reference's scheduler after step_count optimizer steps (last_epoch = k * N),
+        produced by torch's own LambdaLR so the layout is this torch version's."""
+        lam = self.lr_schedule if self.lr_schedule is not None else ConstantLR()
+        base = [self.lr * g["lr_mult"] for g in self._group_def]
+        dummy = torch.optim.AdamW([dict(params=[torch.zeros(1)], lr=b) for b in base])
+        sched = torch.optim.lr_scheduler.LambdaLR(dummy, [lam] * len(base))
+        sched.last_epoch = self.step_count * self.num_processes
+        sched._step_count = sched.last_epoch + 1
+        sched._last_lr = self.get_last_lr()
+        sd = sched.state_dict()
+        if isinstance(lam, ConstantLR):
+            sd["lr_lambdas"] = [None] * len(base)      # diffusers' constant schedule is a plain lambda: torch stores None
+        return sd
+
+    def save_state(self, output_dir):
+        """accelerator.save_state(output_dir) of the recipes: rank 0 writes unet/ (save_pretrained), unet_ema/ (with
+        use_ema), optimizer.bin (torch.optim.AdamW.state_dict() layout), scheduler.bin (LambdaLR.state_dict() layout)
+        and flat_trainer.pt (the device state block: loss scale, growth tracker, applied / skipped counts; step and
+        EMA counts, world size, the group definition); every rank writes random_states_{rank}.pkl (python, numpy,
+        torch CPU and CUDA generator states).  Only at an accumulation-window boundary.  The device buffers go to the
+        host one at a time; no extra device copy is made.  Ends with a barrier when torch.distributed is up."""
+        import os
+        import random
+        import numpy as np
+        import torch.distributed as dist
+        self._check_boundary("save_state")
+        distributed = dist.is_available() and dist.is_initialized()
+        rank = dist.get_rank() if distributed else 0
+        os.makedirs(output_dir, exist_ok=True)
+        if rank == 0:
+            self.module.save_pretrained(os.path.join(output_dir, "unet"))
+            if self.ema is not None:
+                self.save_ema(os.path.join(output_dir, "unet_ema"))
+            state_host = self.state.to("cpu", copy=True)
+            applied = int(state_host[2])
+            opt = dict(state={}, param_groups=self._torch_param_groups())
+            if applied > 0:                   # torch keeps no per-parameter state before a parameter's first update
+                where = {name: (off, shape) for name, off, shape in self._layout}
+                m = self.exp_avg.to("cpu", copy=True)
+                v = self.exp_avg_sq.to("cpu", copy=True)
+                for i, (_, name) in enumerate(self._torch_order()):
+                    off, shape = where[name]
+                    n = math.prod(shape)
+                    opt["state"][i] = dict(step=torch.tensor(float(applied)), exp_avg=m[off:off + n].view(shape),
+                                           exp_avg_sq=v[off:off + n].view(shape))
+                del m, v
+            torch.save(opt, os.path.join(output_dir, "optimizer.bin"))
+            del opt
+            torch.save(self._scheduler_state_dict(), os.path.join(output_dir, "scheduler.bin"))
+            torch.save(dict(state=state_host, step_count=self.step_count, ema_steps=self.ema_steps, world=self.world,
+                            num_processes=self.num_processes, groups=self._group_def),
+                       os.path.join(output_dir, "flat_trainer.pt"))
+        rng = dict(random_state=random.getstate(), numpy_random_seed=np.random.get_state(),
+                   torch_manual_seed=torch.get_rng_state())
+        if torch.cuda.is_available():
+            rng["torch_cuda_manual_seed"] = torch.cuda.get_rng_state_all()
+        torch.save(rng, os.path.join(output_dir, f"random_states_{rank}.pkl"))
+        if distributed:
+            dist.barrier()
+
+    def load_state(self, input_dir):
+        """accelerator.load_state(input_dir): restores the weights, Adam moments, device state block, step / schedule
+        position, the EMA (with use_ema) and this rank's RNG states, bumps the weights epoch (packed fp16 weights and
+        CUDA graphs are rebuilt) and returns the checkpoint's global step (optimizer steps taken).  A folder the
+        reference wrote (no flat_trainer.pt) loads with the trainer's initial loss scale and applied steps = the
+        optimizer's `step`.  Everything is read and checked first: mismatched parameter names or shapes, another
+        group definition, or per-parameter `step` values that differ raise ValueError before any buffer changes.
+        random_states_{rank}.pkl holds numpy's state and is unpickled in full: load only checkpoints you trust."""
+        import os
+        import random
+        import numpy as np
+        import torch.distributed as dist
+        from .modules import bump_weights_epoch
+        self._check_boundary("load_state")
+        path = lambda f: os.path.join(input_dir, f)                               # noqa: E731
+        ft = torch.load(path("flat_trainer.pt"), map_location="cpu") if os.path.exists(path("flat_trainer.pt")) else None
+        if ft is not None and ft["groups"] != self._group_def:
+            raise ValueError(f"{input_dir}: saved with parameter groups "
+                             f"{[(g['name'], g['lr_mult'], g['weight_decay'], len(g['params'])) for g in ft['groups']]}, "
+                             f"this trainer has {[(g['name'], g['lr_mult'], g['weight_decay'], len(g['params'])) for g in self._group_def]}")
+        weights = self._load_checked(path("unet"), "parameter")
+        opt = torch.load(path("optimizer.bin"), map_location="cpu")
+        pg = opt["param_groups"]
+        if [len(g["params"]) for g in pg] != [len(g["params"]) for g in self._group_def] or \
+                [float(g["weight_decay"]) for g in pg] != [g["weight_decay"] for g in self._group_def]:
+            raise ValueError(f"{input_dir}: the optimizer's parameter groups (sizes "
+                             f"{[len(g['params']) for g in pg]}) differ from this trainer's "
+                             f"({[len(g['params']) for g in self._group_def]})")
+        order = self._torch_order()
+        index_of = [i for g in pg for i in g["params"]]
+        shapes = {name: shape for name, _, shape in self._layout}
+        steps, moments = set(), ({}, {})
+        for pos, i in enumerate(index_of):
+            st = opt["state"].get(i)
+            name = order[pos][1]
+            steps.add(float(st["step"]) if st is not None else 0.0)
+            if st is not None:
+                for d, key in zip(moments, ("exp_avg", "exp_avg_sq")):
+                    if tuple(st[key].shape) != shapes[name]:
+                        raise ValueError(f"{input_dir}: optimizer state of {name} has shape {list(st[key].shape)}, "
+                                         f"the parameter {list(shapes[name])}")
+                    d[name] = st[key]
+        if len(steps) > 1:
+            raise ValueError(f"{input_dir}: per-parameter AdamW steps {sorted(steps)} differ; the fused optimizer keeps "
+                             "one step count (one bias correction) for all parameters")
+        applied = int(steps.pop()) if steps else 0
+        sched = torch.load(path("scheduler.bin"), map_location="cpu") if os.path.exists(path("scheduler.bin")) else None
+        if ft is not None:
+            step_count, state = int(ft["step_count"]), ft["state"].float()
+        else:
+            step_count = int(sched["last_epoch"]) // self.num_processes if sched is not None else applied
+            state = torch.tensor([self._init_loss_scale, 0, applied, 0, 0, 0, 0, 0], dtype=torch.float32)
+        ema = self._read_ema(path("unet_ema")) if self.ema is not None else None
+        rank = dist.get_rank() if (dist.is_available() and dist.is_initialized()) else 0
+        rng_file = path(f"random_states_{rank}.pkl")
+        rng = torch.load(rng_file, weights_only=False) if os.path.exists(rng_file) else None
+        # everything checked: write
         with torch.no_grad():
-            for name, off, shape in self._layout:
-                if name not in sd or tuple(sd[name].shape) != shape:
-                    raise ValueError(f"{directory}: no EMA weight {name} of shape {list(shape)}")
-                n = sd[name].numel()
-                self.ema[off:off + n].copy_(sd[name].reshape(-1))
-        self.ema_steps = step
+            self.flat_param.copy_(self._flat_from(weights))
+            del weights
+            for buf, d in zip((self.exp_avg, self.exp_avg_sq), moments):
+                buf.copy_(self._flat_from(d) if d else torch.zeros(buf.numel()))
+            self.state.copy_(state)
+            if ema is not None:
+                self.ema.copy_(ema[1])
+                self.ema_steps = ema[0]
+            self.flat_grad.zero_()
+        self.step_count, self._micro, self._synced = step_count, 0, True
+        if rng is not None:
+            random.setstate(rng["random_state"])
+            np.random.set_state(rng["numpy_random_seed"])
+            torch.set_rng_state(rng["torch_manual_seed"])
+            if "torch_cuda_manual_seed" in rng and torch.cuda.is_available():
+                torch.cuda.set_rng_state_all(rng["torch_cuda_manual_seed"])
+        bump_weights_epoch()
+        return step_count
 
     # ---- host read-backs (each one is a device sync: for logging / tests, not for the training loop)
     def loss_scale(self):

@@ -246,6 +246,24 @@ int b200_adamw_step_state(float* param, const float* grad, float* exp_avg, float
                           const double* grad_norm_sq, float max_grad_norm, float inv_world, float* state,
                           int dynamic_scale, float growth_interval, float min_scale, float max_scale, void* stream);
 
+/* Per-group learning rates (ABI 11): torch.optim.AdamW with parameter groups, e.g. GeoWizard's two groups of
+ * train_depth_normal.py:428-444 (every `class_embedding.*` parameter at learning_rate * class_embedding_lr_mult) or
+ * Marigold's one group of training/train.py:346-353.  The flat buffer is cut into n_runs RUNS: run r covers elements
+ * [run_start[r], run_start[r+1]) (the last one up to n) and belongs to group run_group[r]; run_start (int64) and
+ * run_group (int32) live on the DEVICE, run_start[0] == 0, starts increase and are multiples of 4.  group_lr /
+ * group_wd are HOST arrays of n_groups values, passed with the launch.  With n_runs == 1 the tables may be NULL (the
+ * whole buffer is group 0).  Everything else, the state block and its single skip decision / loss scale / bias
+ * correction included, is b200_adamw_step_state's (which is this call with one run).  Per element the arithmetic is
+ * unchanged: decay = 1 - lr*wd, step_size = lr / bc1 of the element's group. */
+#define B200_ADAMW_MAX_GROUPS 16
+#define B200_ADAMW_MAX_RUNS 1024
+int b200_adamw_step_state_groups(float* param, const float* grad, float* exp_avg, float* exp_avg_sq, long long n,
+                                 const long long* run_start, const int* run_group, int n_runs, const float* group_lr,
+                                 const float* group_wd, int n_groups, float beta1, float beta2, float eps,
+                                 const double* grad_norm_sq, float max_grad_norm, float inv_world, float* state,
+                                 int dynamic_scale, float growth_interval, float min_scale, float max_scale,
+                                 void* stream);
+
 /* ---- Backward pass (training/train.py:545-566, `accelerator.backward(loss)`).  The GEMM-shaped halves run on
  * b200_linear / b200_conv2d_nhwc with re-packed operands; these are the streaming / reduction kernels around them.
  *
