@@ -86,6 +86,12 @@ int sm_count() {
   return n[dev];
 }
 
+// Debug record of the last gemm_conv_kernel launch (b200_debug_last_launch): which instantiation ran and on which tile
+// geometry, so tests can assert the path and tile they mean to cover.  Written by launch_one only; never read on the
+// launch path.  Field order: include/b200_e2eft.h.
+constexpr int kLastLaunchFields = 16;
+static int g_last_launch[kLastLaunchFields] = {0};
+
 // ------------------------------------------------------------------------------------------
 template <int BN, typename OutT, bool SWAP, bool GEGLU = false, bool HALO = false, bool VEC = false>
 static int launch_one(const CUtensorMap& a, const CUtensorMap& a2, const CUtensorMap& b,
@@ -108,6 +114,12 @@ static int launch_one(const CUtensorMap& a, const CUtensorMap& a2, const CUtenso
   // fused statistics are carried across a CTA's tiles while (image, channel tile) stays the same: with the channel tile
   // fastest in the tile index, a grid that is a multiple of n_tiles keeps every CTA on ONE channel tile
   if (SWAP && p.chan_stats && p.n_tiles > 1 && grid > p.n_tiles) grid -= grid % p.n_tiles;
+  {
+    const int rec[kLastLaunchFields] = {p.conv, HALO, SWAP, BN, VEC, GEGLU, (int)std::is_same<OutT, float>::value,
+                                        p.bw, p.bh, p.halo_n, p.tiles_w, p.tiles_h, p.m_tiles, p.n_tiles, grid,
+                                        p.chan_stats != nullptr};
+    memcpy(g_last_launch, rec, sizeof(rec));
+  }
   kern<<<grid, kGemmThreads, S::kTotalBytes, st>>>(a, a2, b, p);
   B200_CHECK_LAUNCH("gemm_conv_kernel");
   return 0;
@@ -197,7 +209,13 @@ extern "C" void b200_debug_set_flags(int f) { b200::g_debug = f; }
 extern "C" void b200_debug_set_swap(int m) { b200::g_swap_mode = m; }
 extern "C" void b200_debug_set_halo(int m) { b200::g_halo_mode = m; }
 extern "C" int b200_debug_last_path(void) { return b200::g_last_path; }
-extern "C" int b200_abi_version(void) { return 11; }
+extern "C" int b200_debug_last_launch(int* out, int n) {
+  if (!out || n <= 0) return kLastLaunchFields;
+  const int k = n < kLastLaunchFields ? n : kLastLaunchFields;
+  memcpy(out, b200::g_last_launch, k * sizeof(int));
+  return kLastLaunchFields;
+}
+extern "C" int b200_abi_version(void) { return 12; }
 // Tile width used by the GEGLU epilogue for a packed width N (= 2 x output width); weights must be
 // packed per tile as [value half | gate half] with this width.
 extern "C" int b200_geglu_block_n(int N) {

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 11        # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 12        # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -23,6 +23,7 @@ _SIGS = {
     "b200_debug_set_swap": (None, [c_int]),
     "b200_debug_set_halo": (None, [c_int]),
     "b200_debug_last_path": (c_int, []),
+    "b200_debug_last_launch": (c_int, [POINTER(c_int), c_int]),
     "b200_geglu_block_n": (c_int, [c_int]),
     "b200_linear": (c_int, [_P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_int, _P, c_int, _P, _LL, _LL,
                             _P, _LL, _LL, c_int, c_int, c_float, _P, c_int, _P, c_int, c_int, c_int, _LL, _P]),

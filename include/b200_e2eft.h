@@ -331,6 +331,12 @@ void b200_debug_set_flags(int flags);
 void b200_debug_set_swap(int mode);
 void b200_debug_set_halo(int mode);   /* 1 = automatic halo-resident stride-1 3x3 conv (default), 0 = per-tap boxes */
 int b200_debug_last_path(void);       /* path of the last b200_conv2d_nhwc call: 1 = halo-resident, 0 = per-tap boxes */
+/* Record of the last gemm_conv_kernel launch, from b200_linear or b200_conv2d_nhwc (ABI 12): which template instantiation
+ * ran and on which tile geometry.  Copies min(n, 16) ints to out and returns 16 (the record length; out may be NULL).
+ * Fields: 0 conv (1) / linear (0), 1 halo-resident, 2 swapped orientation, 3 BLOCK_N, 4 vectorised epilogue (VEC),
+ * 5 GEGLU, 6 fp32 output, 7 bw, 8 bh, 9 halo_n (halo MMA width), 10 tiles_w, 11 tiles_h, 12 m_tiles, 13 n_tiles,
+ * 14 grid (CTAs), 15 fused statistics.  Debug only: nothing on the launch path reads it. */
+int b200_debug_last_launch(int* out, int n);
 
 /* torchvision resize(x, size, BICUBIC, antialias=True) of [planes][H][W] fp32 (aten _upsample_bicubic2d_aa, Keys
  * cubic a = -0.5): the CLIP image-encoder input of GeoWizard/geowizard/models/geowizard_pipeline.py:239-243.
