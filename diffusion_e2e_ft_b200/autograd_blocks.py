@@ -1,9 +1,11 @@
 """Training-mode (differentiable) execution of the engine blocks — SURVEY.md §8 row a10.
 
 The reference trains through `accelerator.backward(loss)` (training/train.py:563): plain torch.autograd over
-the UNet and the frozen VAE decoder.  The engine keeps that boundary: every block of modules.py / unet.py is one
-`torch.autograd.Function` whose forward runs the same sm_90a kernels as inference (saving the operands the
-backward needs) and whose backward is hand-written on the backward operators of backward.py / csrc/backward.cu.
+the UNet and the frozen VAE decoder.  The engine keeps that boundary: every block of modules.py / unet.py / vae.py is
+one `torch.autograd.Function`.  Its forward calls the block's inference forward (`forward_saved`, which also returns
+the intermediates the backward reads) and adds only the GroupNorm mean / rstd of the saved inputs; its backward is
+hand-written on the backward operators of backward.py / csrc/backward.cu and reads the weights through the same
+`_packed*` methods as inference.  So a training forward launches the inference kernels by construction.
 torch.autograd is used for what it is in the reference — graph bookkeeping between blocks (skip connections,
 the shared time embedding, `.grad` accumulation) — never for arithmetic inside a block.
 
@@ -37,10 +39,9 @@ def _stash(out, box):
     return out
 
 
-def _bwd_cache(mod):
-    if not hasattr(mod, "_pk_bwd"):
-        mod._pk_bwd = Packed()
-    return mod._pk_bwd
+def _bwd_cache(mod, kind=""):
+    """The module's cache of the backward operand `kind` (re-packed weights), built by one function."""
+    return mod.__dict__.setdefault("_pk_bwd", {}).setdefault(kind, Packed())
 
 
 def _any(ctx, first):
@@ -57,28 +58,14 @@ def _resnet_params(m):
 
 
 class _ResnetFn(torch.autograd.Function):
-    """ResnetBlock2D.run + its backward.  inputs: x [NB,H,W,C1] fp32, skip [NB,H,W,C2] | None, temb [NB,cout] | None."""
+    """ResnetBlock2D + its backward.  inputs: x [NB,H,W,C1] fp32, skip [NB,H,W,C2] | None, temb [NB,cout] | None."""
 
     @staticmethod
     def run(m, f16_copy, x, skip, temb):
-        pk = m._packed()
-        xs = [x] if skip is None else [x, skip]
+        out, (a1, raw, h, a2) = m.forward_saved(x, temb, skip, F32, f16_copy)
         mr1 = ops.group_norm_mean_rstd(x, m.eps, m.groups, skip)
-        raw = None
-        if m.conv_shortcut is not None:
-            a1, raw = ops.group_norm(x, pk["g1"], pk["b1"], m.eps, m.groups, True, x2=skip, want_raw=True)
-        else:
-            assert skip is None
-            a1 = ops.group_norm(x, pk["g1"], pk["b1"], m.eps, m.groups, True)
-        h = ops.conv2d(a1, pk["w1"], m.cout, bias=pk["c1b"], rowvec=temb, stats=True)
         mr2 = ops.group_norm_mean_rstd(h, m.eps, m.groups)
-        a2 = ops.group_norm(h, pk["g2"], pk["b2"], m.eps, m.groups, True)
-        if raw is not None:
-            out = ops.conv2d(a2, pk["w2"], m.cout, bias=pk["c2b"], x2=raw, out_dtype=F32, stats=True, f16_copy=f16_copy)
-        else:
-            out = ops.conv2d(a2, pk["w2"], m.cout, bias=pk["c2b"], residual=x, out_dtype=F32, stats=True,
-                             f16_copy=f16_copy)
-        return out, (xs, mr1, a1, raw, h, mr2, a2)
+        return out, ([x] if skip is None else [x, skip], mr1, a1, raw, h, mr2, a2)
 
     @staticmethod
     def forward(ctx, m, f16_copy, box, x, skip, temb, *params):
@@ -159,15 +146,8 @@ def resnet(m, x, temb=None, skip=None, f16_copy=False, ckpt=False):
 class _DownsampleFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, m, box, x, weight, bias):
-        pk = m._pk.get(list(m.parameters()), lambda: dict(w=ops.pack_conv(m.conv.weight), b=_f32(m.conv.bias)))
-        NB, H, W, C = x.shape
-        if m.padding == 1:
-            taps, Ho, Wo = TAPS3, (H - 1) // 2 + 1, (W - 1) // 2 + 1
-        else:
-            taps, Ho, Wo = TAPS3_PAD0, (H - 2) // 2 + 1, (W - 2) // 2 + 1
-        x16 = ops.cast_f16(x)
-        out = ops.conv2d(x16, pk["w"], C, bias=pk["b"], taps=taps, stride=2, out_hw=(Ho, Wo), out_dtype=F32, stats=True)
-        ctx.m, ctx.saved, ctx.taps = m, (x16,), taps
+        out, x16 = m.forward_saved(x)
+        ctx.m, ctx.saved = m, (x16,)
         return _stash(out, box)
 
     @staticmethod
@@ -175,12 +155,12 @@ class _DownsampleFn(torch.autograd.Function):
         m = ctx.m
         (x16,) = ctx.saved
         NB, H, W, C = x16.shape
+        taps, kind = (TAPS3, "s2") if m.padding == 1 else (TAPS3_PAD0, "s2_vae")
         d16 = ops.cast_f16(dout.contiguous())
         gw = gb = None
         if _any(ctx, 3):
-            dwp, gb = bw.conv_wgrad(x16, d16, ctx.taps, stride=2)
+            dwp, gb = bw.conv_wgrad(x16, d16, taps, stride=2)
             gw = bw.unpack_conv_grad(dwp, C)
-        kind = "s2" if m.padding == 1 else "s2_vae"
         pb = _bwd_cache(m).get([m.conv.weight], lambda: pack_conv_dgrad_s2(m.conv.weight, 1 if m.padding == 1 else 0))
         dx = bw.conv_dgrad(d16, None, C, kind, out_dtype=F32, packed=pb, in_hw=(H, W))
         return None, None, dx, gw, gb
@@ -192,75 +172,39 @@ def downsample(m, x):
 
 
 class _UpsampleFn(torch.autograd.Function):
-    """nearest-2x + conv3x3 as four 2x2 phase convs (Upsample2D.run, default size)."""
-
-    @staticmethod
-    def forward(ctx, m, box, x, weight, bias):
-        pk = m._pk.get(list(m.parameters()), lambda: dict(ph=m._pack_phases(), b=_f32(m.conv.bias)))
-        NB, H, W, C = x.shape
-        x16 = ops.cast_f16(x)
-        out = torch.empty((NB, 2 * H, 2 * W, C), dtype=F32, device=x.device)
-        cs = ops._new_stats(NB, C, x.device) if ops.FUSE_GN_STATS else None
-        for (py, px), (taps, wp) in pk["ph"].items():
-            ops.conv2d(x16, wp, C, bias=pk["b"], taps=taps, out_hw=(H, W), out=out, out_mul=2, out_off=(py, px), stats=cs)
-        if cs is not None:
-            out._cs = cs
-        ctx.m, ctx.saved = m, (x16,)
-        return _stash(out, box)
-
-    @staticmethod
-    def backward(ctx, dout):
-        m = ctx.m
-        (x16,) = ctx.saved
-        C = x16.shape[3]
-        d16 = ops.cast_f16(dout.contiguous())
-        gw = gb = None
-        if _any(ctx, 3):
-            dwp, gb = bw.conv_wgrad(x16, d16, TAPS3, up=2)
-            gw = bw.unpack_conv_grad(dwp, C)
-        pb = _bwd_cache(m).get([m.conv.weight], lambda: dict(up=pack_upsample_conv_dgrad(m._pack_phases())))
-        if "up" not in pb:
-            pb["up"] = pack_upsample_conv_dgrad(m._pack_phases())
-        dx = bw.conv_dgrad(d16, None, C, "up", out_dtype=F32, packed=pb["up"])
-        return None, None, dx, gw, gb
-
-
-class _UpsampleSizeFn(torch.autograd.Function):
-    """nearest upsample to an explicit size (unet_2d_condition.py:1185-1186, latent sizes not divisible by
-    2^levels) + conv3x3: Upsample2D.run's second branch."""
+    """Upsample2D + its backward: nearest-2x + conv3x3 as four 2x2 phase convs, or nearest to an explicit size
+    (unet_2d_condition.py:1185-1186, latent sizes not divisible by 2^levels) + conv3x3."""
 
     @staticmethod
     def forward(ctx, m, out_hw, box, x, weight, bias):
-        pk = m._pk2.get(list(m.parameters()), lambda: dict(w=ops.pack_conv(m.conv.weight), b=_f32(m.conv.bias)))
-        C = x.shape[3]
-        up = ops.upsample_nearest(x, out_hw)
-        out = ops.conv2d(up, pk["w"], C, bias=pk["b"], out_dtype=F32, stats=True)
-        ctx.m, ctx.saved, ctx.in_hw = m, (up,), tuple(x.shape[1:3])
+        out, a = m.forward_saved(x, out_hw)
+        ctx.m, ctx.saved, ctx.in_hw, ctx.resize = m, (a,), tuple(x.shape[1:3]), m.resizes(x, out_hw)
         return _stash(out, box)
 
     @staticmethod
     def backward(ctx, dout):
         m = ctx.m
-        (up,) = ctx.saved
-        C = up.shape[3]
+        (a,) = ctx.saved
+        C = a.shape[3]
         d16 = ops.cast_f16(dout.contiguous())
         gw = gb = None
         if _any(ctx, 4):
-            dwp, gb = bw.conv_wgrad(up, d16, TAPS3)
+            dwp, gb = bw.conv_wgrad(a, d16, TAPS3, up=1 if ctx.resize else 2)
             gw = bw.unpack_conv_grad(dwp, C)
-        pb = _bwd_cache(m).get([m.conv.weight], lambda: dict(s1=pack_conv_dgrad_s1(m.conv.weight)))
-        if "s1" not in pb:
-            pb["s1"] = pack_conv_dgrad_s1(m.conv.weight)
-        dup = bw.conv_dgrad(d16, None, C, "s1", out_dtype=F32, packed=pb["s1"])
-        return None, None, None, ops.upsample_nearest_bwd(dup, ctx.in_hw), gw, gb
+        if ctx.resize:
+            pb = _bwd_cache(m, "s1").get([m.conv.weight], lambda: pack_conv_dgrad_s1(m.conv.weight))
+            da = bw.conv_dgrad(d16, None, C, "s1", out_dtype=F32, packed=pb)
+            dx = ops.upsample_nearest_bwd(da, ctx.in_hw)
+        else:
+            pb = _bwd_cache(m, "up").get([m.conv.weight],
+                                         lambda: pack_upsample_conv_dgrad(m._packed_phases()["ph"]))
+            dx = bw.conv_dgrad(d16, None, C, "up", out_dtype=F32, packed=pb)
+        return None, None, None, dx, gw, gb
 
 
 def upsample(m, x, out_hw=None):
-    NB, H, W, C = x.shape
     box = {}
-    if out_hw is not None and tuple(out_hw) != (2 * H, 2 * W):
-        return _attach(_UpsampleSizeFn.apply(m, tuple(out_hw), box, x, m.conv.weight, m.conv.bias), box)
-    return _attach(_UpsampleFn.apply(m, box, x, m.conv.weight, m.conv.bias), box)
+    return _attach(_UpsampleFn.apply(m, out_hw, box, x, m.conv.weight, m.conv.bias), box)
 
 
 # ---------------------------------------------------------------------------------------- transformer block
@@ -277,54 +221,20 @@ def _transformer_params(m):
 
 
 class _TransformerFn(torch.autograd.Function):
-    """Transformer2DModel.run (one BasicTransformerBlock; plain or GeoWizard joint self-attention) + its backward."""
+    """Transformer2DModel (one BasicTransformerBlock; plain or GeoWizard joint self-attention) + its backward."""
 
     @staticmethod
     def run(m, f16_copy, x, ctx16):
-        blk = m.transformer_blocks[0]
-        own = [m.norm.weight, m.norm.bias, m.proj_in.weight, m.proj_in.bias, m.proj_out.weight, m.proj_out.bias]
-        pk = m._pk.get(own, lambda: dict(g=_f32(m.norm.weight), b=_f32(m.norm.bias),
-                                         wi=_f16(m.proj_in.weight), bi=_f32(m.proj_in.bias),
-                                         wo=_f16(m.proj_out.weight), bo=_f32(m.proj_out.bias)))
-        bp = blk._packed()
-        B, H, W, C = x.shape
-        L, heads, scale = H * W, blk.heads, 64 ** -0.5
+        out, (hn, h0, blk_saved, h16) = m.forward_saved(x, ctx16, F32, f16_copy)     # general path: no const_ctx
         mr0 = ops.group_norm_mean_rstd(x, 1e-6, m.groups)
-        hn = ops.group_norm(x, pk["g"], pk["b"], 1e-6, m.groups, False)
-        h0 = ops.linear(hn.view(B * L, C), pk["wi"], pk["bi"], out_dtype=F32)
-        n1 = ops.layer_norm(h0, *bp["ln"][0])
-        qkv = ops.linear(n1, bp["wqkv"]).view(B, L, 3 * C)
-        o = ops.attention_d64(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, scale,
-                              kv_segments=2 if blk.joint else 1)
-        h1 = ops.linear(o.view(B * L, C), bp["wo1"], bp["bo1"], residual=h0, out_dtype=F32)
-        n2 = ops.layer_norm(h1, *bp["ln"][1])
-        q2 = ops.linear(n2, bp["wq2"]).view(B, L, C)
-        S = ctx16.shape[1]
-        c2d = ctx16.reshape(B * S, -1)
-        kv = ops.linear(c2d, bp["wkv2"]).view(B, S, 2 * C)
-        o2 = ops.attention_d64(q2, kv[..., :C], kv[..., C:], heads, scale)
-        h2 = ops.linear(o2.view(B * L, C), bp["wo2"], bp["bo2"], residual=h1, out_dtype=F32)
-        n3 = ops.layer_norm(h2, *bp["ln"][2])
-        gate = ops.linear(n3, bp["wgt"], bp["bgt"], act=ops.ACT_GELU)
-        gg = ops.linear(n3, bp["wv"], bp["bv"], residual=gate, res_mul=True)
-        h3 = ops.linear(gg, bp["wf"], bp["bf"], residual=h2, out_dtype=F32, f16_copy=True)
-        h16 = ops.cast_f16(h3)
-        out = ops.linear(h16, pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=F32, stats_rows_per_img=L,
-                         f16_copy=f16_copy)
-        return out, (x, mr0, hn, h0, n1, qkv, o, h1, n2, q2, c2d, kv, o2, h2, n3, gg, h16)
+        return out, (x, mr0, hn, h0, *blk_saved, h16)
 
     @staticmethod
     def forward(ctx, m, f16_copy, box, x, ctx16, *params):
         out, saved = _TransformerFn.run(m, f16_copy, x, ctx16)
         ctx.m = m
         ctx.saved, ctx.inputs = (None, (f16_copy, x, ctx16)) if box.get("ckpt") else (saved, None)
-        B, H, W, C = x.shape
-        res = out.view(B, H, W, C)
-        for k in ("_cs", "_h16"):
-            v = getattr(out, k, None)
-            if v is not None:
-                box[k] = v if k == "_cs" else v.view(B, H, W, C)
-        return res
+        return _stash(out, box)
 
     @staticmethod
     def backward(ctx, dout):
@@ -332,7 +242,7 @@ class _TransformerFn(torch.autograd.Function):
         blk = m.transformer_blocks[0]
         saved = ctx.saved if ctx.saved is not None else _TransformerFn.run(m, *ctx.inputs)[1]
         x, mr0, hn, h0, n1, qkv, o, h1, n2, q2, c2d, kv, o2, h2, n3, gg, h16 = saved
-        pk, bp = m._pk._val, blk._packed()
+        pk, bp = m._packed(), blk._packed()
         B, H, W, C = x.shape
         L, heads, scale = H * W, blk.heads, 64 ** -0.5
         S = kv.shape[1]
@@ -404,35 +314,24 @@ def transformer(m, x, ctx16, f16_copy=False, ckpt=False):
 
 # ------------------------------------------------------------------------------------- conv_in / conv_out
 class _ConvInFn(torch.autograd.Function):
-    """ConvInSmall.run: im2col + GEMM from the NCHW sample; backward = weight/bias gradients (the sample is data)
+    """ConvInSmall (im2col + GEMM from the NCHW sample); backward = weight/bias gradients (the sample is data)
     and, when the input needs it (VAE decoder), the data gradient through the small-Cout conv kernel."""
 
     @staticmethod
     def forward(ctx, runner, box, x_nchw, weight, bias):
-        conv = runner.conv
-        cin, cout = conv.weight.shape[1], conv.weight.shape[0]
-        kpad = (9 * cin + 7) // 8 * 8
-        pk = runner._pk.get([conv.weight, conv.bias],
-                            lambda: dict(w=ops.pack_conv_small_cin(conv.weight, kpad), b=_f32(conv.bias)))
-        NB, _, H, W = x_nchw.shape
-        patches = ops.im2col3x3(x_nchw.contiguous(), kpad)
-        out = ops.linear(patches, pk["w"], pk["b"], out_dtype=F32, stats_rows_per_img=H * W)
-        ctx.runner, ctx.saved, ctx.geom = runner, (patches,), (NB, H, W, cin, cout, kpad)
-        cs = getattr(out, "_cs", None)
-        if cs is not None:
-            box["_cs"] = cs
-        return out.view(NB, H, W, cout)
+        out, patches = runner.forward_saved(x_nchw)
+        ctx.runner, ctx.saved, ctx.cin = runner, (patches,), x_nchw.shape[1]
+        return _stash(out, box)
 
     @staticmethod
     def backward(ctx, dout):
-        conv = ctx.runner.conv
+        conv, cin = ctx.runner.conv, ctx.cin
         (patches,) = ctx.saved
-        NB, H, W, cin, cout, kpad = ctx.geom
+        NB, H, W, cout = dout.shape
         d16 = ops.cast_f16(dout.contiguous()).view(NB * H * W, cout)
         gw = gb = dx = None
         if ctx.needs_input_grad[3] or ctx.needs_input_grad[4]:
-            pk = ctx.runner._pk._val
-            _, dwp, gb = bw.linear_bwd(patches, pk["w"], d16, need_da=False)
+            _, dwp, gb = bw.linear_bwd(patches, ctx.runner._packed(cin)["w"], d16, need_da=False)
             gw = dwp[:, :9 * cin].reshape(cout, 3, 3, cin).permute(0, 3, 1, 2).contiguous()
         if ctx.needs_input_grad[2]:
             wq = _bwd_cache(ctx.runner).get([conv.weight], lambda: ops.pack_conv_small_cout(
@@ -447,22 +346,12 @@ def conv_in(runner, x_nchw):
 
 
 class _ConvOutFn(torch.autograd.Function):
-    """ConvOutSmall.run: GroupNorm+SiLU -> conv3x3 with tiny Cout, NCHW fp32 out."""
+    """ConvOutSmall: GroupNorm+SiLU -> conv3x3 with tiny Cout, NCHW fp32 out."""
 
     @staticmethod
     def forward(ctx, runner, x, nw, nb, weight, bias):
-        norm, conv = runner.norm, runner.conv
-        cout, cin = conv.weight.shape[0], conv.weight.shape[1]
-        direct = cout <= 8 and cin % 64 == 0
-        pk = runner._pk.get([norm.weight, norm.bias, conv.weight, conv.bias],
-                            lambda: dict(g=_f32(norm.weight), b=_f32(norm.bias), cb=_f32(conv.bias),
-                                         w=ops.pack_conv_small_cout(conv.weight) if direct else ops.pack_conv(conv.weight)))
-        mr = ops.group_norm_mean_rstd(x, norm.eps, norm.num_groups)
-        a = ops.group_norm(x, pk["g"], pk["b"], norm.eps, norm.num_groups, True)
-        if direct:
-            out = ops.conv3x3_small_cout(a, pk["w"], pk["cb"], cout)
-        else:
-            out = ops.conv2d(a, pk["w"], cout, bias=pk["cb"], out_dtype=F32, out_nchw=True)
+        out, a = runner.forward_saved(x)
+        mr = ops.group_norm_mean_rstd(x, runner.norm.eps, runner.norm.num_groups)
         ctx.runner, ctx.saved = runner, (x, mr, a)
         return out
 
@@ -470,7 +359,7 @@ class _ConvOutFn(torch.autograd.Function):
     def backward(ctx, dout):
         norm, conv = ctx.runner.norm, ctx.runner.conv
         x, mr, a = ctx.saved
-        pk = ctx.runner._pk._val
+        pk = ctx.runner._packed()
         NB, H, W, C = x.shape
         cout = conv.weight.shape[0]
         dout = dout.contiguous().float()
@@ -507,23 +396,13 @@ def _embed_params(unet):
 
 class _EmbedFn(torch.autograd.Function):
     """sinusoid -> linear_1 -> SiLU -> linear_2 (+ class embedding) -> SiLU -> every resnet's time_emb_proj in one GEMM
-    (unet.py forward, unet_2d_condition.py:957-1000)."""
+    (B200UNet2DConditionModel._time_embedding, unet_2d_condition.py:957-1000)."""
 
     @staticmethod
     def forward(ctx, unet, t, class_labels, *params):
-        ep = unet._embed_packed()
-        B = t.shape[0]
-        e0 = ops.timestep_embedding(t, unet.config["block_out_channels"][0])
-        e1 = ops.linear(e0, ep["w1"], ep["b1"], act=ops.ACT_SILU)
-        cl = c1 = c = None
-        if unet.class_embedding is not None:
-            cl = torch.zeros((B, ep["ckpad"]), dtype=F16, device=t.device)
-            cl[:, :class_labels.shape[1]] = class_labels
-            c1 = ops.linear(cl, ep["cw1"], ep["cb1"], act=ops.ACT_SILU)
-            c = ops.linear(c1, ep["cw2"], ep["cb2"])
-        e2 = ops.linear(e1, ep["w2"], ep["b2"], residual=c, act=ops.ACT_SILU)
-        ctx.unet, ctx.saved = unet, (e0, e1, e2, cl, c1, c)
-        return ops.linear(e2, ep["wall"], ep["ball"], out_dtype=F32)
+        out, ctx.saved = unet._time_embedding(t, class_labels)
+        ctx.unet = unet
+        return out
 
     @staticmethod
     def backward(ctx, dall):
@@ -554,42 +433,21 @@ def embed(unet, t, class_labels):
 
 # ------------------------------------------------------------------------------------ VAE mid-block attention
 class _VAEAttentionFn(torch.autograd.Function):
-    """VAEAttention.run (single head, d = channels) + its data gradient.  The VAE is frozen in the fine-tuning
-    recipe (training/train.py:323-326), so only d/dx is produced."""
+    """VAEAttention's unfused path (single head, d = channels) + its data gradient.  The VAE is frozen in the
+    fine-tuning recipe (training/train.py:323-326), so only d/dx is produced."""
 
     @staticmethod
     def forward(ctx, m, box, x):
-        pk = m._pk.get(list(m.parameters()), lambda: dict(
-            g=_f32(m.group_norm.weight), b=_f32(m.group_norm.bias),
-            wqk=_f16(torch.cat([m.to_q.weight, m.to_k.weight], 0)),
-            bqk=_f32(torch.cat([m.to_q.bias, m.to_k.bias], 0)),
-            wv=_f16(m.to_v.weight), bv=_f32(m.to_v.bias),
-            wo=_f16(m.to_out[0].weight), bo=_f32(m.to_out[0].bias)))
-        B, H, W, C = x.shape
-        L = H * W
-        Lp = ops._ru8(L)
+        out, (hn, qk, p_buf, o) = m.forward_unfused(x)
         mr = ops.group_norm_mean_rstd(x, m.eps, m.groups)
-        hn = ops.group_norm(x, pk["g"], pk["b"], m.eps, m.groups, False).view(B, L, C)
-        qk = ops.linear(hn.view(B * L, C), pk["wqk"], pk["bqk"]).view(B, L, 2 * C)
-        vt_buf = torch.empty((B, C, Lp), dtype=F16, device=x.device)
-        vt = ops.linear(pk["wv"], hn, pk["bv"], bias_row=True, out=vt_buf[:, :, :L])
-        s_buf = torch.empty((B, L, Lp), dtype=F32, device=x.device)
-        ops.linear(qk[..., :C], qk[..., C:], out=s_buf[:, :, :L])
-        p_buf = ops.softmax_rows(s_buf, C ** -0.5, cols=L)
-        o = ops.linear(p_buf[:, :, :L], vt)
-        out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=F32,
-                         stats_rows_per_img=L)
         ctx.m, ctx.saved = m, (x, mr, hn, qk, p_buf, o)
-        cs = getattr(out, "_cs", None)
-        if cs is not None:
-            box["_cs"] = cs
-        return out.view(B, H, W, C)
+        return _stash(out, box)
 
     @staticmethod
     def backward(ctx, dout):
         m = ctx.m
         x, mr, hn, qk, p_buf, o = ctx.saved
-        pk = m._pk._val
+        pk = m._packed()
         if any(p.requires_grad for p in m.parameters()):
             raise NotImplementedError("the VAE attention block is differentiable w.r.t. its input only (frozen VAE)")
         B, H, W, C = x.shape

@@ -114,6 +114,10 @@ class ResnetBlock2D(nn.Module):
     def run(self, x, temb=None, skip=None, sdt=F32, f16_copy=False):
         """x (and optional skip, channel-concatenated after x): stream NHWC; temb: fp32 [B,cout] view.
         `f16_copy`: the output also gets an fp16 twin (the next op is a stride-2 / upsample conv)."""
+        return self.forward_saved(x, temb, skip, sdt, f16_copy)[0]
+
+    def forward_saved(self, x, temb=None, skip=None, sdt=F32, f16_copy=False):
+        """`run`, also returning the intermediates its backward reads: (out, (a1, raw, h, a2))."""
         pk = self._packed()
         if self.conv_shortcut is not None and (skip is not None or x.dtype != F16):
             # the 1x1 shortcut needs the (concatenated) input as an fp16 operand: emitted by the GN pass
@@ -125,10 +129,12 @@ class ResnetBlock2D(nn.Module):
         h = ops.conv2d(a1, pk["w1"], self.cout, bias=pk["c1b"], rowvec=temb, stats=True)
         a2 = ops.group_norm(h, pk["g2"], pk["b2"], self.eps, self.groups, True)
         if raw is not None:
-            return ops.conv2d(a2, pk["w2"], self.cout, bias=pk["c2b"], x2=raw, out_dtype=sdt, stats=True,
-                              f16_copy=f16_copy)
-        return ops.conv2d(a2, pk["w2"], self.cout, bias=pk["c2b"], residual=x, out_dtype=sdt, stats=True,
-                          f16_copy=f16_copy)
+            out = ops.conv2d(a2, pk["w2"], self.cout, bias=pk["c2b"], x2=raw, out_dtype=sdt, stats=True,
+                             f16_copy=f16_copy)
+        else:
+            out = ops.conv2d(a2, pk["w2"], self.cout, bias=pk["c2b"], residual=x, out_dtype=sdt, stats=True,
+                             f16_copy=f16_copy)
+        return out, (a1, raw, h, a2)
 
 
 class Downsample2D(nn.Module):
@@ -140,17 +146,25 @@ class Downsample2D(nn.Module):
         self.conv = nn.Conv2d(ch, ch, 3, stride=2, padding=padding)
         self._pk = Packed()
 
+    def _packed(self):
+        return self._pk.get(list(self.parameters()),
+                            lambda: dict(w=ops.pack_conv(self.conv.weight), b=_f32(self.conv.bias)))
+
     def run(self, x, sdt=F32):
-        pk = self._pk.get(list(self.parameters()),
-                          lambda: dict(w=ops.pack_conv(self.conv.weight), b=_f32(self.conv.bias)))
+        return self.forward_saved(x, sdt)[0]
+
+    def forward_saved(self, x, sdt=F32):
+        """`run`, also returning the fp16 conv operand its weight gradient reads: (out, x16)."""
+        pk = self._packed()
         NB, H, W, C = x.shape
         if self.padding == 1:
             taps, Ho, Wo = ops.TAPS3, (H - 1) // 2 + 1, (W - 1) // 2 + 1
         else:
             taps, Ho, Wo = ops.TAPS3_PAD0, (H - 2) // 2 + 1, (W - 2) // 2 + 1
         x16 = x if x.dtype == F16 else ops.cast_f16(x)
-        return ops.conv2d(x16, pk["w"], C, bias=pk["b"], taps=taps, stride=2, out_hw=(Ho, Wo), out_dtype=sdt,
-                          stats=True)
+        out = ops.conv2d(x16, pk["w"], C, bias=pk["b"], taps=taps, stride=2, out_hw=(Ho, Wo), out_dtype=sdt,
+                         stats=True)
+        return out, x16
 
 
 class Upsample2D(nn.Module):
@@ -183,22 +197,37 @@ class Upsample2D(nn.Module):
                 out[(py, px)] = (taps, wp)
         return out
 
+    def _packed_phases(self):
+        return self._pk.get(list(self.parameters()), lambda: dict(ph=self._pack_phases(), b=_f32(self.conv.bias)))
+
+    def _packed_resize(self):
+        return self._pk2.get(list(self.parameters()),
+                             lambda: dict(w=ops.pack_conv(self.conv.weight), b=_f32(self.conv.bias)))
+
+    @staticmethod
+    def resizes(x, out_hw):
+        """True when `out_hw` is not the exact 2x of x: nearest resize to out_hw, then a plain conv3x3."""
+        return out_hw is not None and tuple(out_hw) != (2 * x.shape[1], 2 * x.shape[2])
+
     def run(self, x, out_hw=None, sdt=F32):
+        return self.forward_saved(x, out_hw, sdt)[0]
+
+    def forward_saved(self, x, out_hw=None, sdt=F32):
+        """`run`, also returning the fp16 conv operand its weight gradient reads: (out, x16) for the exact 2x,
+        (out, resized input) otherwise."""
         NB, H, W, C = x.shape
-        if out_hw is None or tuple(out_hw) == (2 * H, 2 * W):
-            pk = self._pk.get(list(self.parameters()),
-                              lambda: dict(ph=self._pack_phases(), b=_f32(self.conv.bias)))
+        if not self.resizes(x, out_hw):
+            pk = self._packed_phases()
             x16 = x if x.dtype == F16 else ops.cast_f16(x)
             out = torch.empty((NB, 2 * H, 2 * W, C), dtype=sdt, device=x.device)
             cs = ops._new_stats(NB, C, x.device) if ops.FUSE_GN_STATS else None
             for (py, px), (taps, wp) in pk["ph"].items():
                 ops.conv2d(x16, wp, C, bias=pk["b"], taps=taps, out_hw=(H, W), out=out, out_mul=2, out_off=(py, px),
                            stats=cs)
-            return out
-        pk = self._pk2.get(list(self.parameters()),
-                           lambda: dict(w=ops.pack_conv(self.conv.weight), b=_f32(self.conv.bias)))
+            return out, x16
+        pk = self._packed_resize()
         up = ops.upsample_nearest(x, out_hw)
-        return ops.conv2d(up, pk["w"], C, bias=pk["b"], out_dtype=sdt, stats=True)
+        return ops.conv2d(up, pk["w"], C, bias=pk["b"], out_dtype=sdt, stats=True), up
 
 
 # ------------------------------------------------------------------------------------ attention
@@ -291,34 +320,40 @@ class BasicTransformerBlock(nn.Module):
                 wf=_f16(self.ff.net[2].weight), bf=_f32(self.ff.net[2].bias))
         return self._pk.get(list(self.parameters()), build)
 
-    def run(self, h, B, L, ctx16, sdt=F32, const_ctx=None):
-        """h: stream [B*L, C]; ctx16: fp16 [B, S, Dctx]; const_ctx: [S, Dctx] when all images share one context."""
+    def forward_saved(self, h0, B, L, ctx16, sdt=F32, const_ctx=None, save=True):
+        """h0: stream [B*L, C]; ctx16: fp16 [B, S, Dctx]; const_ctx: [S, Dctx] when all images share one context.
+        Returns (out, saved): `saved` holds the intermediates the backward reads, None unless `save`."""
+        assert not (save and const_ctx is not None), "the backward exists for the general cross-attention path only"
         pk = self._packed()
         C, heads = self.dim, self.heads
         scale = 64 ** -0.5
-        n1 = ops.layer_norm(h, *pk["ln"][0])
+        n1 = ops.layer_norm(h0, *pk["ln"][0])
         qkv = ops.linear(n1, pk["wqkv"]).view(B, L, 3 * C)
         o = ops.attention_d64(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, scale,
                               kv_segments=2 if self.joint else 1)
-        h = ops.linear(o.view(B * L, C), pk["wo1"], pk["bo1"], residual=h, out_dtype=sdt)
-        n2 = ops.layer_norm(h, *pk["ln"][1])
+        h1 = ops.linear(o.view(B * L, C), pk["wo1"], pk["bo1"], residual=h0, out_dtype=sdt)
+        n2 = ops.layer_norm(h1, *pk["ln"][1])
         S = ctx16.shape[1]
         if const_ctx is not None and heads * S <= self.CONST_CTX_MAX_J:
             cc = self._packed_const_ctx(const_ctx)
             lg = ops.linear(n2, cc["a16"], out_dtype=F32)                              # [B*L, Jp] scaled logits
             p2 = ops.softmax_groups(lg, heads, S, cc["Jp"])
-            h = ops.linear(p2, cc["vwt16"], pk["bo2"], residual=h, out_dtype=sdt)
+            h2 = ops.linear(p2, cc["vwt16"], pk["bo2"], residual=h1, out_dtype=sdt)
         else:
             q2 = ops.linear(n2, pk["wq2"]).view(B, L, C)
-            kv = ops.linear(ctx16.reshape(B * S, -1), pk["wkv2"]).view(B, S, 2 * C)
+            c2d = ctx16.reshape(B * S, -1)
+            kv = ops.linear(c2d, pk["wkv2"]).view(B, S, 2 * C)
             o2 = ops.attention_d64(q2, kv[..., :C], kv[..., C:], heads, scale)
-            h = ops.linear(o2.view(B * L, C), pk["wo2"], pk["bo2"], residual=h, out_dtype=sdt)
-        n3 = ops.layer_norm(h, *pk["ln"][2])
+            h2 = ops.linear(o2.view(B * L, C), pk["wo2"], pk["bo2"], residual=h1, out_dtype=sdt)
+        saved = (n1, qkv, o, h1, n2, q2, c2d, kv, o2) if save else None
+        del h1                          # without `save`, the feed-forward below runs with h1 already freed
+        n3 = ops.layer_norm(h2, *pk["ln"][2])
         # GEGLU (attention.py:754-755) as two swapped-operand GEMMs: gate = gelu(x Wg + bg), then
         # value = (x Wv + bv) * gate in the second epilogue (the fused single-GEMM variant is barrier-bound)
         gate = ops.linear(n3, pk["wgt"], pk["bgt"], act=ops.ACT_GELU)
         g = ops.linear(n3, pk["wv"], pk["bv"], residual=gate, res_mul=True)
-        return ops.linear(g, pk["wf"], pk["bf"], residual=h, out_dtype=sdt, f16_copy=True)   # proj_out operand
+        out = ops.linear(g, pk["wf"], pk["bf"], residual=h2, out_dtype=sdt, f16_copy=True)   # proj_out operand
+        return out, None if saved is None else (*saved, h2, n3, g)
 
 
 class Transformer2DModel(nn.Module):
@@ -334,22 +369,29 @@ class Transformer2DModel(nn.Module):
         self.proj_out = nn.Linear(dim, dim)
         self._pk = Packed()
 
-    def run(self, x, ctx16, sdt=F32, f16_copy=False, const_ctx=None):
+    def _packed(self):
         own = [self.norm.weight, self.norm.bias, self.proj_in.weight, self.proj_in.bias,
                self.proj_out.weight, self.proj_out.bias]
-        pk = self._pk.get(own, lambda: dict(g=_f32(self.norm.weight), b=_f32(self.norm.bias),
-                                            wi=_f16(self.proj_in.weight), bi=_f32(self.proj_in.bias),
-                                            wo=_f16(self.proj_out.weight), bo=_f32(self.proj_out.bias)))
+        return self._pk.get(own, lambda: dict(g=_f32(self.norm.weight), b=_f32(self.norm.bias),
+                                              wi=_f16(self.proj_in.weight), bi=_f32(self.proj_in.bias),
+                                              wo=_f16(self.proj_out.weight), bo=_f32(self.proj_out.bias)))
+
+    def run(self, x, ctx16, sdt=F32, f16_copy=False, const_ctx=None):
+        return self.forward_saved(x, ctx16, sdt, f16_copy, const_ctx, save=False)[0]
+
+    def forward_saved(self, x, ctx16, sdt=F32, f16_copy=False, const_ctx=None, save=True):
+        """`run`, also returning the intermediates its backward reads: (out, (hn, h0, block saved, h16))."""
+        pk = self._packed()
+        (blk,) = self.transformer_blocks
         B, H, W, C = x.shape
         L = H * W
         hn = ops.group_norm(x, pk["g"], pk["b"], 1e-6, self.groups, False)
-        h = ops.linear(hn.view(B * L, C), pk["wi"], pk["bi"], out_dtype=sdt)
-        for blk in self.transformer_blocks:
-            h = blk.run(h, B, L, ctx16, sdt, const_ctx)
+        h0 = ops.linear(hn.view(B * L, C), pk["wi"], pk["bi"], out_dtype=sdt)
+        h, saved = blk.forward_saved(h0, B, L, ctx16, sdt, const_ctx, save)
         h16 = h if h.dtype == F16 else ops.cast_f16(h)
         out = ops.linear(h16, pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt, stats_rows_per_img=L,
                          f16_copy=f16_copy)
-        return _view_cs(out, B, H, W, C)
+        return _view_cs(out, B, H, W, C), (hn, h0, saved, h16)
 
 
 # ------------------------------------------------------------------------------------ small-Cin conv
@@ -360,21 +402,29 @@ class ConvInSmall:
         self.conv = conv
         self._pk = Packed()
 
+    def _packed(self, cin):
+        """Weights for an input carrying the first `cin` channels: dict(w [cout, kpad] fp16, b, kpad)."""
+        conv = self.conv
+        kpad = (9 * cin + 7) // 8 * 8
+        pks = self.__dict__.setdefault("_pks", {})
+        return pks.setdefault(cin, Packed()).get(
+            [conv.weight, conv.bias],
+            lambda: dict(w=ops.pack_conv_small_cin(conv.weight[:, :cin], kpad), b=_f32(conv.bias), kpad=kpad))
+
     def run(self, x_nchw, sdt=F32):
         """x_nchw may carry only the LEADING channels of the layer's input: the missing trailing channels are exact
         zeros (single-step zeros-noise path, marigold_pipeline.py:418-423,447-449: conv_in on 4 of the 8 channels)."""
-        conv = self.conv
-        cout = conv.weight.shape[0]
-        cin = x_nchw.shape[1]
-        assert cin <= conv.weight.shape[1]
-        kpad = (9 * cin + 7) // 8 * 8
-        pks = self.__dict__.setdefault("_pks", {})
-        pk = pks.setdefault(cin, Packed()).get(
-            [conv.weight, conv.bias],
-            lambda: dict(w=ops.pack_conv_small_cin(conv.weight[:, :cin], kpad), b=_f32(conv.bias)))
-        NB, _, H, W = x_nchw.shape
-        patches = ops.im2col3x3(x_nchw.contiguous(), kpad)
-        return _view_cs(ops.linear(patches, pk["w"], pk["b"], out_dtype=sdt, stats_rows_per_img=H * W), NB, H, W, cout)
+        return self.forward_saved(x_nchw, sdt)[0]
+
+    def forward_saved(self, x_nchw, sdt=F32):
+        """`run`, also returning the im2col patches its weight gradient reads: (out, patches)."""
+        cout = self.conv.weight.shape[0]
+        NB, cin, H, W = x_nchw.shape
+        assert cin <= self.conv.weight.shape[1]
+        pk = self._packed(cin)
+        patches = ops.im2col3x3(x_nchw.contiguous(), pk["kpad"])
+        out = ops.linear(patches, pk["w"], pk["b"], out_dtype=sdt, stats_rows_per_img=H * W)
+        return _view_cs(out, NB, H, W, cout), patches
 
 
 class ConvOutSmall:
@@ -384,14 +434,21 @@ class ConvOutSmall:
         self.norm, self.conv = norm, conv
         self._pk = Packed()
 
-    def run(self, x):
+    def _packed(self):
         norm, conv = self.norm, self.conv
-        cout, cin = conv.weight.shape[0], conv.weight.shape[1]
-        direct = cout <= 8 and cin % 64 == 0
-        pk = self._pk.get([norm.weight, norm.bias, conv.weight, conv.bias],
-                          lambda: dict(g=_f32(norm.weight), b=_f32(norm.bias), cb=_f32(conv.bias),
-                                       w=ops.pack_conv_small_cout(conv.weight) if direct else ops.pack_conv(conv.weight)))
+        direct = conv.weight.shape[0] <= 8 and conv.weight.shape[1] % 64 == 0
+        return self._pk.get([norm.weight, norm.bias, conv.weight, conv.bias],
+                            lambda: dict(g=_f32(norm.weight), b=_f32(norm.bias), cb=_f32(conv.bias), direct=direct,
+                                         w=ops.pack_conv_small_cout(conv.weight) if direct else ops.pack_conv(conv.weight)))
+
+    def run(self, x):
+        return self.forward_saved(x)[0]
+
+    def forward_saved(self, x):
+        """`run`, also returning the normalised conv operand its backward reads: (out, a)."""
+        norm, cout = self.norm, self.conv.weight.shape[0]
+        pk = self._packed()
         a = ops.group_norm(x, pk["g"], pk["b"], norm.eps, norm.num_groups, True)
-        if direct:
-            return ops.conv3x3_small_cout(a, pk["w"], pk["cb"], cout)      # input read once (halo tile in smem)
-        return ops.conv2d(a, pk["w"], cout, bias=pk["cb"], out_dtype=F32, out_nchw=True)
+        if pk["direct"]:
+            return ops.conv3x3_small_cout(a, pk["w"], pk["cb"], cout), a      # input read once (halo tile in smem)
+        return ops.conv2d(a, pk["w"], cout, bias=pk["cb"], out_dtype=F32, out_nchw=True), a

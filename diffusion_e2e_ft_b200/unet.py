@@ -11,6 +11,7 @@ diffusers `state_dict` names (SURVEY.md App. A.8).  All arithmetic runs in libb2
 import torch
 import torch.nn as nn
 
+from . import autograd_blocks as ab
 from . import ops
 from .modules import (ConfigDict, ConvInSmall, ConvOutSmall, Downsample2D, Packed, ResnetBlock2D,
                       Transformer2DModel, Upsample2D, _f16, _f32)
@@ -199,34 +200,67 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
     #     (modules.BasicTransformerBlock._packed_const_ctx).
     single_step_specialisations = True
 
-    def _time_embedding(self, t, class_labels, B, dev):
-        """[B, sum(cout)] fp32: every resnet's time_emb_proj(silu(temb (+class_emb))) (unet_2d_condition.py:957-1000)."""
-        cfg = self.config
+    def _time_embedding(self, t, class_labels):
+        """[B, sum(cout)] fp32: every resnet's time_emb_proj(silu(temb (+class_emb))) (unet_2d_condition.py:957-1000),
+        and the intermediates its backward reads: (out, (e0, e1, e2, cl, c1, c))."""
         ep = self._embed_packed()
-        e = ops.timestep_embedding(t, cfg["block_out_channels"][0])
-        e = ops.linear(e, ep["w1"], ep["b1"], act=ops.ACT_SILU)
+        e0 = ops.timestep_embedding(t, self.config["block_out_channels"][0])
+        e1 = ops.linear(e0, ep["w1"], ep["b1"], act=ops.ACT_SILU)
+        cl = c1 = c = None
         if self.class_embedding is not None:
-            if class_labels is None:
-                raise ValueError("class_labels should be provided when num_class_embeds > 0")
-            cl = torch.zeros((B, ep["ckpad"]), dtype=F16, device=dev)
+            cl = torch.zeros((t.shape[0], ep["ckpad"]), dtype=F16, device=t.device)
             cl[:, :class_labels.shape[1]] = class_labels
-            c = ops.linear(cl, ep["cw1"], ep["cb1"], act=ops.ACT_SILU)
-            c = ops.linear(c, ep["cw2"], ep["cb2"])
-            e = ops.linear(e, ep["w2"], ep["b2"], residual=c, act=ops.ACT_SILU)     # silu(temb + class_emb)
-        else:
-            e = ops.linear(e, ep["w2"], ep["b2"], act=ops.ACT_SILU)                 # silu(temb)
-        return ops.linear(e, ep["wall"], ep["ball"], out_dtype=F32)                  # all 22 time_emb_proj at once
+            c1 = ops.linear(cl, ep["cw1"], ep["cb1"], act=ops.ACT_SILU)
+            c = ops.linear(c1, ep["cw2"], ep["cb2"])
+        e2 = ops.linear(e1, ep["w2"], ep["b2"], residual=c, act=ops.ACT_SILU)         # silu(temb (+ class_emb))
+        return ops.linear(e2, ep["wall"], ep["ball"], out_dtype=F32), (e0, e1, e2, cl, c1, c)   # all 22 time_emb_proj
+
+    def _walk(self, x, temb_of, forward_size, resnet, transformer, downsample, upsample):
+        """Down / mid / up blocks from conv_in's output to conv_norm_out's input (unet_2d_condition.py:1005-1206).
+        The four steps run one block each, as inference modules or as autograd Functions:
+        resnet(block, x, temb, skip, f16_copy), transformer(block, x, f16_copy), downsample(block, x),
+        upsample(block, x, out_hw)."""
+        skips = [x]
+        for blk in self.down_blocks:
+            for i, r in enumerate(blk.resnets):
+                last = (i == len(blk.resnets) - 1) and blk.downsamplers is not None    # feeds the stride-2 conv
+                x = resnet(r, x, temb_of[id(r)], None, last and blk.attentions is None)
+                if blk.attentions is not None:
+                    x = transformer(blk.attentions[i], x, last)
+                skips.append(x)
+            if blk.downsamplers is not None:
+                x = downsample(blk.downsamplers[0], x)
+                skips.append(x)
+        mb = self.mid_block
+        x = resnet(mb.resnets[0], x, temb_of[id(mb.resnets[0])], None, False)
+        x = transformer(mb.attentions[0], x, False)
+        x = resnet(mb.resnets[1], x, temb_of[id(mb.resnets[1])], None, False)
+        for blk in self.up_blocks:
+            for i, r in enumerate(blk.resnets):
+                skip = skips.pop()
+                last = (i == len(blk.resnets) - 1) and blk.upsamplers is not None and not forward_size
+                x = resnet(r, x, temb_of[id(r)], skip, last and blk.attentions is None)
+                if blk.attentions is not None:
+                    x = transformer(blk.attentions[i], x, last)
+            if blk.upsamplers is not None:
+                x = upsample(blk.upsamplers[0], x, tuple(skips[-1].shape[1:3]) if forward_size else None)
+        return x
 
     def forward(self, sample, timestep, encoder_hidden_states, class_labels=None, return_dict=True, **unused):
+        """With grad enabled and a parameter or `sample` requiring grad, every block runs as its autograd Function
+        (autograd_blocks.py), so `loss.backward()` fills `.grad` like the reference's training/train.py:563."""
         ops._need_cuda(sample)                                                      # sm_90a only, no CPU fallback
-        if torch.is_grad_enabled() and (sample.requires_grad or any(p.requires_grad for p in self.parameters())):
-            return self._forward_train(sample, timestep, encoder_hidden_states, class_labels, return_dict)
+        train = torch.is_grad_enabled() and (sample.requires_grad or any(p.requires_grad for p in self.parameters()))
         cfg, sdt = self.config, self.stream_dtype
+        if train and sdt != F32:
+            raise NotImplementedError("training runs with the fp32 residual stream (stream_dtype=torch.float32)")
+        if self.class_embedding is not None and class_labels is None:
+            raise ValueError("class_labels should be provided when num_class_embeds > 0")
         B, _, H, W = sample.shape
         dev = sample.device
         n_up = len(cfg["block_out_channels"]) - 1
         forward_size = (H % (2 ** n_up) != 0) or (W % (2 ** n_up) != 0)      # unet_2d_condition.py:920-930
-        spec = self.single_step_specialisations
+        spec = self.single_step_specialisations and not train
         if sample.shape[1] != cfg["in_channels"] and not (spec and sample.shape[1] < cfg["in_channels"]):
             raise ValueError(f"sample has {sample.shape[1]} channels, conv_in expects {cfg['in_channels']}")
 
@@ -238,7 +272,7 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
             temb_all = cache.get(key)
             if temb_all is None:
                 t = torch.full((B,), float(timestep), dtype=F32, device=dev)
-                temb_all = cache[key] = self._time_embedding(t, None, B, dev)
+                temb_all = cache[key] = self._time_embedding(t, None)[0]
                 if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
                     cache.pop(key)                                   # graph-private memory must not outlive the capture
         else:
@@ -246,113 +280,37 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
                 t = torch.full((B,), float(timestep), dtype=F32, device=dev)
             else:
                 t = timestep.to(device=dev, dtype=F32).reshape(-1).expand(B).contiguous()
-            temb_all = self._time_embedding(t, class_labels, B, dev)
+            temb_all = ab.embed(self, t, class_labels) if train else self._time_embedding(t, class_labels)[0]
         resnets = list(self._resnets())
         temb_of = {id(r): temb_all[:, o:o + r.cout] for r, o in zip(resnets, ep["offs"])}
 
-        ehs = encoder_hidden_states
+        ehs = encoder_hidden_states.detach()
         const_ctx = None
         if spec and ehs.dim() == 3 and (ehs.shape[0] == 1 or ehs.stride(0) == 0):
             const_ctx = ehs[0]                                      # [S, Dctx] shared by every image
         ctx16 = ehs.to(F16).contiguous()
 
-        # ---- down path
         if not hasattr(self, "_conv_in_run") or self._conv_in_run.conv is not self.conv_in:
             self._conv_in_run = ConvInSmall(self.conv_in)       # conv_in may be swapped (unet_prep.py:6-21)
-        x = self._conv_in_run.run(sample if sample.dtype in (F16, F32) else sample.float(), sdt)
-        skips = [x]
-        for blk in self.down_blocks:
-            for i, r in enumerate(blk.resnets):
-                last = (i == len(blk.resnets) - 1) and blk.downsamplers is not None    # feeds the stride-2 conv
-                x = r.run(x, temb_of[id(r)], None, sdt, f16_copy=last and blk.attentions is None)
-                if blk.attentions is not None:
-                    x = blk.attentions[i].run(x, ctx16, sdt, f16_copy=last, const_ctx=const_ctx)
-                skips.append(x)
-            if blk.downsamplers is not None:
-                x = blk.downsamplers[0].run(x, sdt)
-                skips.append(x)
-        # ---- mid
-        mb = self.mid_block
-        x = mb.resnets[0].run(x, temb_of[id(mb.resnets[0])], None, sdt)
-        x = mb.attentions[0].run(x, ctx16, sdt, const_ctx=const_ctx)
-        x = mb.resnets[1].run(x, temb_of[id(mb.resnets[1])], None, sdt)
-        # ---- up path
-        for bi, blk in enumerate(self.up_blocks):
-            for i, r in enumerate(blk.resnets):
-                skip = skips.pop()
-                last = (i == len(blk.resnets) - 1) and blk.upsamplers is not None and not forward_size
-                x = r.run(x, temb_of[id(r)], skip, sdt, f16_copy=last and blk.attentions is None)
-                if blk.attentions is not None:
-                    x = blk.attentions[i].run(x, ctx16, sdt, f16_copy=last, const_ctx=const_ctx)
-            if blk.upsamplers is not None:
-                size = tuple(skips[-1].shape[1:3]) if forward_size else None
-                x = blk.upsamplers[0].run(x, size, sdt)
-        # ---- out
         if not hasattr(self, "_conv_out_run") or self._conv_out_run.conv is not self.conv_out:
             self._conv_out_run = ConvOutSmall(self.conv_norm_out, self.conv_out)
-        out = self._conv_out_run.run(x)
-        if out.dtype != sample.dtype:
-            out = out.to(sample.dtype)
-        if not return_dict:
-            return (out,)
-        return UNet2DConditionOutput(out)
-
-
-    # ------------------------------------------------------------------ differentiable forward (row a10)
-    def _forward_train(self, sample, timestep, encoder_hidden_states, class_labels, return_dict):
-        """Same graph as `forward`, every block executed as a torch.autograd.Function (autograd_blocks.py) so
-        `loss.backward()` fills `.grad` of the parameters exactly like the reference's training/train.py:563."""
-        from . import autograd_blocks as ab
-        ck = bool(self._gradient_checkpointing)
-        if self.stream_dtype != F32:
-            raise NotImplementedError("training runs with the fp32 residual stream (stream_dtype=torch.float32)")
-        cfg = self.config
-        B, _, H, W = sample.shape
-        dev = sample.device
-        n_up = len(cfg["block_out_channels"]) - 1
-        forward_size = (H % (2 ** n_up) != 0) or (W % (2 ** n_up) != 0)      # unet_2d_condition.py:920-930
-        if not torch.is_tensor(timestep):
-            t = torch.full((B,), float(timestep), dtype=F32, device=dev)
+        x_in = sample if sample.dtype in (F16, F32) else sample.float()
+        if train:
+            ck = bool(self._gradient_checkpointing)
+            x = ab.conv_in(self._conv_in_run, x_in.detach())
+            x = self._walk(x, temb_of, forward_size,
+                           lambda r, x, temb, skip, f16_copy: ab.resnet(r, x, temb, skip, f16_copy, ckpt=ck),
+                           lambda m, x, f16_copy: ab.transformer(m, x, ctx16, f16_copy, ckpt=ck),
+                           ab.downsample, ab.upsample)
+            out = ab.conv_out(self._conv_out_run, x)
         else:
-            t = timestep.to(device=dev, dtype=F32).reshape(-1).expand(B).contiguous()
-        if self.class_embedding is not None and class_labels is None:
-            raise ValueError("class_labels should be provided when num_class_embeds > 0")
-        temb_all = ab.embed(self, t, class_labels)
-        ep = self._embed_packed()
-        resnets = list(self._resnets())
-        temb_of = {id(r): temb_all[:, o:o + r.cout] for r, o in zip(resnets, ep["offs"])}
-        ctx16 = encoder_hidden_states.detach().to(F16).contiguous()
-
-        if not hasattr(self, "_conv_in_run") or self._conv_in_run.conv is not self.conv_in:
-            self._conv_in_run = ConvInSmall(self.conv_in)
-        x = ab.conv_in(self._conv_in_run, (sample if sample.dtype in (F16, F32) else sample.float()).detach())
-        skips = [x]
-        for blk in self.down_blocks:
-            for i, r in enumerate(blk.resnets):
-                last = (i == len(blk.resnets) - 1) and blk.downsamplers is not None
-                x = ab.resnet(r, x, temb_of[id(r)], None, f16_copy=last and blk.attentions is None, ckpt=ck)
-                if blk.attentions is not None:
-                    x = ab.transformer(blk.attentions[i], x, ctx16, f16_copy=last, ckpt=ck)
-                skips.append(x)
-            if blk.downsamplers is not None:
-                x = ab.downsample(blk.downsamplers[0], x)
-                skips.append(x)
-        mb = self.mid_block
-        x = ab.resnet(mb.resnets[0], x, temb_of[id(mb.resnets[0])], ckpt=ck)
-        x = ab.transformer(mb.attentions[0], x, ctx16, ckpt=ck)
-        x = ab.resnet(mb.resnets[1], x, temb_of[id(mb.resnets[1])], ckpt=ck)
-        for blk in self.up_blocks:
-            for i, r in enumerate(blk.resnets):
-                skip = skips.pop()
-                last = (i == len(blk.resnets) - 1) and blk.upsamplers is not None and not forward_size
-                x = ab.resnet(r, x, temb_of[id(r)], skip, f16_copy=last and blk.attentions is None, ckpt=ck)
-                if blk.attentions is not None:
-                    x = ab.transformer(blk.attentions[i], x, ctx16, f16_copy=last, ckpt=ck)
-            if blk.upsamplers is not None:
-                x = ab.upsample(blk.upsamplers[0], x, tuple(skips[-1].shape[1:3]) if forward_size else None)
-        if not hasattr(self, "_conv_out_run") or self._conv_out_run.conv is not self.conv_out:
-            self._conv_out_run = ConvOutSmall(self.conv_norm_out, self.conv_out)
-        out = ab.conv_out(self._conv_out_run, x)
+            x = self._conv_in_run.run(x_in, sdt)
+            x = self._walk(x, temb_of, forward_size,
+                           lambda r, x, temb, skip, f16_copy: r.run(x, temb, skip, sdt, f16_copy),
+                           lambda m, x, f16_copy: m.run(x, ctx16, sdt, f16_copy, const_ctx),
+                           lambda m, x: m.run(x, sdt),
+                           lambda m, x, out_hw: m.run(x, out_hw, sdt))
+            out = self._conv_out_run.run(x)
         if out.dtype != sample.dtype:
             out = out.to(sample.dtype)
         if not return_dict:

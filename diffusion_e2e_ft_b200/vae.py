@@ -9,6 +9,7 @@ Graph per SURVEY.md App. A.6 (blocks shaped as GeoWizard/geowizard/models/unet_2
 import torch
 import torch.nn as nn
 
+from . import autograd_blocks as ab
 from . import ops
 from .modules import (ConfigDict, ConvInSmall, ConvOutSmall, Downsample2D, Packed, ResnetBlock2D,
                       Upsample2D, _f16, _f32, _view_cs)
@@ -59,8 +60,8 @@ class VAEAttention(nn.Module):
         self._pk = Packed()
         self.memory_efficient = False       # B200AutoencoderKL.enable_xformers_memory_efficient_attention
 
-    def run(self, x, sdt=F32):
-        pk = self._pk.get(list(self.parameters()), lambda: dict(
+    def _packed(self):
+        return self._pk.get(list(self.parameters()), lambda: dict(
             g=_f32(self.group_norm.weight), b=_f32(self.group_norm.bias),
             wqk=_f16(torch.cat([self.to_q.weight, self.to_k.weight], 0)),
             bqk=_f32(torch.cat([self.to_q.bias, self.to_k.bias], 0)),
@@ -68,27 +69,41 @@ class VAEAttention(nn.Module):
             wqkv=_f16(torch.cat([self.to_q.weight, self.to_k.weight, self.to_v.weight], 0)),
             bqkv=_f32(torch.cat([self.to_q.bias, self.to_k.bias, self.to_v.bias], 0)),
             wo=_f16(self.to_out[0].weight), bo=_f32(self.to_out[0].bias)))
+
+    def run(self, x, sdt=F32):
+        B, H, W, C = x.shape
+        if use_fused_attention(B, H * W, C, self.memory_efficient):
+            return self.forward_fused(x, sdt)
+        return self.forward_unfused(x, sdt)[0]
+
+    def forward_fused(self, x, sdt=F32):
+        pk = self._packed()
         B, H, W, C = x.shape
         L = H * W
-        if use_fused_attention(B, L, C, self.memory_efficient):
-            hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B * L, C)
-            qkv = ops.linear(hn, pk["wqkv"], pk["bqkv"]).view(B, L, 3 * C)
-            o = ops.attention_d512(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], C ** -0.5)   # [B, L, C]
-            out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt,
-                             stats_rows_per_img=L)
-            return _view_cs(out, B, H, W, C)
+        hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B * L, C)
+        qkv = ops.linear(hn, pk["wqkv"], pk["bqkv"]).view(B, L, 3 * C)
+        o = ops.attention_d512(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], C ** -0.5)   # [B, L, C]
+        out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt,
+                         stats_rows_per_img=L)
+        return _view_cs(out, B, H, W, C)
+
+    def forward_unfused(self, x, sdt=F32):
+        """The unfused path, also returning the intermediates its backward reads: (out, (hn, qk, p_buf, o))."""
+        pk = self._packed()
+        B, H, W, C = x.shape
+        L = H * W
         Lp = (L + 7) // 8 * 8                       # leading dims must be multiples of 8 elements
         hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B, L, C)
         qk = ops.linear(hn.view(B * L, C), pk["wqk"], pk["bqk"]).view(B, L, 2 * C)
         vt_buf = torch.empty((B, C, Lp), dtype=F16, device=x.device)
         vt = ops.linear(pk["wv"], hn, pk["bv"], bias_row=True, out=vt_buf[:, :, :L])        # V^T [B, C, L]
         s_buf = torch.empty((B, L, Lp), dtype=F32, device=x.device)
-        s = ops.linear(qk[..., :C], qk[..., C:], out=s_buf[:, :, :L])                       # [B, L, L] fp32
+        ops.linear(qk[..., :C], qk[..., C:], out=s_buf[:, :, :L])                           # S [B, L, L] fp32
         p_buf = ops.softmax_rows(s_buf, C ** -0.5, cols=L)
         o = ops.linear(p_buf[:, :, :L], vt)                                                 # [B, L, C]
         out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt,
                          stats_rows_per_img=L)
-        return _view_cs(out, B, H, W, C)
+        return _view_cs(out, B, H, W, C), (hn, qk, p_buf, o)
 
 
 class _MidBlock(nn.Module):
@@ -97,10 +112,11 @@ class _MidBlock(nn.Module):
         self.resnets = nn.ModuleList([ResnetBlock2D(ch, ch, None, groups, eps) for _ in range(2)])
         self.attentions = nn.ModuleList([VAEAttention(ch, groups, eps)])
 
-    def run(self, x, sdt):
-        x = self.resnets[0].run(x, None, None, sdt)
-        x = self.attentions[0].run(x, sdt)
-        return self.resnets[1].run(x, None, None, sdt)
+    def run(self, x, resnet, attention):
+        """resnet(block, x) / attention(block, x): the inference or the differentiable step of each block."""
+        x = resnet(self.resnets[0], x)
+        x = attention(self.attentions[0], x)
+        return resnet(self.resnets[1], x)
 
 
 class _DownEncoderBlock(nn.Module):
@@ -148,12 +164,13 @@ class Encoder(nn.Module):
         _check_input(x, "B200AutoencoderKL.encoder")
         sdt = self.stream_dtype
         h = self._in.run(x if x.dtype in (F16, F32) else x.float(), sdt)
+        resnet = lambda r, h, f16_copy=False: r.run(h, None, None, sdt, f16_copy)         # noqa: E731
         for blk in self.down_blocks:
             for i, r in enumerate(blk.resnets):
-                h = r.run(h, None, None, sdt, f16_copy=(i == len(blk.resnets) - 1 and blk.downsamplers is not None))
+                h = resnet(r, h, i == len(blk.resnets) - 1 and blk.downsamplers is not None)
             if blk.downsamplers is not None:
                 h = blk.downsamplers[0].run(h, sdt)
-        h = self.mid_block.run(h, sdt)
+        h = self.mid_block.run(h, resnet, lambda m, h: m.run(h, sdt))
         out = self._out.run(h)
         return out if out.dtype == x.dtype else out.to(x.dtype)
 
@@ -179,42 +196,31 @@ class Decoder(nn.Module):
         self._out = ConvOutSmall(self.conv_norm_out, self.conv_out)
 
     def forward(self, z):
-        if torch.is_grad_enabled() and z.requires_grad:
-            return self._forward_train(z)
-        _check_input(z, "B200AutoencoderKL.decoder")
+        """With grad enabled and `z.requires_grad` every block runs as its autograd Function (autograd_blocks.py);
+        the VAE is frozen in training (training/train.py:323-326), so only the data gradient is produced."""
+        ops._need_cuda(z)                                  # sm_90a only, no CPU fallback
         sdt = self.stream_dtype
-        h = self._in.run(z if z.dtype in (F16, F32) else z.float(), sdt)
-        h = self.mid_block.run(h, sdt)
+        zin = z if z.dtype in (F16, F32) else z.float()
+        train = torch.is_grad_enabled() and z.requires_grad
+        if train:
+            if sdt != F32:
+                raise NotImplementedError("training runs with the fp32 residual stream (stream_dtype=torch.float32)")
+            h = ab.conv_in(self._in, zin)
+            resnet = lambda r, h, f16_copy=False: ab.resnet(r, h, f16_copy=f16_copy)      # noqa: E731
+            attention, upsample = ab.vae_attention, ab.upsample
+        else:
+            h = self._in.run(zin, sdt)
+            resnet = lambda r, h, f16_copy=False: r.run(h, None, None, sdt, f16_copy)     # noqa: E731
+            attention = lambda m, h: m.run(h, sdt)                                         # noqa: E731
+            upsample = lambda m, h: m.run(h, None, sdt)                                    # noqa: E731
+        h = self.mid_block.run(h, resnet, attention)
         for blk in self.up_blocks:
             for i, r in enumerate(blk.resnets):
-                h = r.run(h, None, None, sdt, f16_copy=(i == len(blk.resnets) - 1 and blk.upsamplers is not None))
+                h = resnet(r, h, i == len(blk.resnets) - 1 and blk.upsamplers is not None)
             if blk.upsamplers is not None:
-                h = blk.upsamplers[0].run(h, None, sdt)
-        out = self._out.run(h)
+                h = upsample(blk.upsamplers[0], h)
+        out = ab.conv_out(self._out, h) if train else self._out.run(h)
         return out if out.dtype == z.dtype else out.to(z.dtype)
-
-
-def _decoder_forward_train(self, z):
-    """Differentiable decoder (row a10): same graph as `Decoder.forward` on the autograd blocks.  With the VAE
-    frozen (training/train.py:323-326) only the data gradient is produced."""
-    from . import autograd_blocks as ab
-    if self.stream_dtype != F32:
-        raise NotImplementedError("training runs with the fp32 residual stream (stream_dtype=torch.float32)")
-    h = ab.conv_in(self._in, z if z.dtype in (F16, F32) else z.float())
-    mb = self.mid_block
-    h = ab.resnet(mb.resnets[0], h)
-    h = ab.vae_attention(mb.attentions[0], h)
-    h = ab.resnet(mb.resnets[1], h)
-    for blk in self.up_blocks:
-        for i, r in enumerate(blk.resnets):
-            h = ab.resnet(r, h, f16_copy=(i == len(blk.resnets) - 1 and blk.upsamplers is not None))
-        if blk.upsamplers is not None:
-            h = ab.upsample(blk.upsamplers[0], h)
-    out = ab.conv_out(self._out, h)
-    return out if out.dtype == z.dtype else out.to(z.dtype)
-
-
-Decoder._forward_train = _decoder_forward_train
 
 
 class Conv1x1Small(nn.Conv2d):
@@ -303,7 +309,6 @@ class B200AutoencoderKL(PretrainedMixin, nn.Module):
         post_quant_conv, decoder  (marigold_pipeline.py:457-465, 513-516)."""
         s = 1.0 / self.config["scaling_factor"]
         if torch.is_grad_enabled() and model_out.requires_grad:
-            from . import autograd_blocks as ab
             if noisy is None or c_noisy == 0.0:
                 return self.decoder(ab.pointwise(self.post_quant_conv, model_out, c_out * s))
             # noisy-start E2E fine-tuning: c_noisy * x_t is a constant addend, so the backward is unchanged

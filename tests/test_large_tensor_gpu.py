@@ -144,7 +144,7 @@ def _run(NB, h, w, seed):
         x = torch.randn(NB, h, w, C, device="cuda", generator=g, dtype=torch.float16)
         # ---- Upsample2D: four phase convs into one fp32 tensor, statistics summed into one buffer
         up = up_m.run(x, None, torch.float32)
-        pk = up_m._pk.get(list(up_m.parameters()), None)
+        pk = up_m._packed_phases()
         bias = pk["b"].double()
         for img, lo, hi in bands:
             ref = torch.empty(hi - lo, W, C, dtype=torch.float64, device="cuda")
