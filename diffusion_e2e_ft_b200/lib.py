@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 12        # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 13       # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -97,6 +97,11 @@ _SIGS = {
     "b200_ema_update": (c_int, [_P, _P, _LL, c_float, _P]),
     "b200_cast_f32_to_f16": (c_int, [_P, _P, _LL, _P]),
     "b200_nhwc_to_nchw_f32": (c_int, [_P, c_int, c_int, c_int, _LL, _P, _P]),
+    "b200_eval_align_depth": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_float, c_int, _P, _P, _P]),
+    "b200_eval_depth_metrics": (c_int, [_P, _P, _P, c_int, _LL, _P, c_int, c_int, c_float, c_float, _P, _P, _P, _P]),
+    "b200_eval_normal_error": (c_int, [_P, POINTER(c_longlong), _P, POINTER(c_longlong), _P, c_int, c_int, c_int, _P,
+                                       _P, _LL, _P, _P, _P, _P, _P]),
+    "b200_eval_kth_smallest": (c_int, [_P, _P, _LL, _LL, _P, _P, _P]),
 }
 EXPORTS = tuple(_SIGS)
 

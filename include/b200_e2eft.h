@@ -414,6 +414,51 @@ int b200_masked_latent_mse_bwd(const void* pred, int pred_f16, const float* targ
                                void* stream);
 int b200_ema_update(float* ema, const float* param, long long n, float one_minus_decay, void* stream);
 
+/* Evaluation of depth and normal predictions (ABI 13).  Every sum is an fp64 partial per block, combined in a fixed
+ * order (no floating-point atomics: two runs give the same bits); counts and indices are 64-bit; nothing syncs the
+ * host.  Maps are fp32, masks bytes (nonzero = valid), all on the device.  `ws` workspaces hold
+ * B x B200_EVAL_MAX_BLOCKS x (7 | 11 | 8) doubles for align_depth / depth_metrics / normal_error.
+ *
+ * b200_eval_align_depth: Marigold/src/util/alignment.py:8-55 (np.linalg.lstsq of [p 1] x = g over the mask) as called
+ *   at Marigold/eval.py:173-203.  gt / pred / mask [B][H][W].  The moments are taken over every row and the columns
+ *   j < OW at source column min(floor(float(j) * col_scale), W - 1): the grid torch.nn.Upsample(scale_factor=s,
+ *   mode="nearest") samples from the [1, H, W] tensor of alignment.py:26 (OW = floor(W * s), col_scale = float(1 / s);
+ *   OW = W for no down-sampling).  disparity: the target is 1 / gt and the mask is mask & gt > 0 & pred > 0
+ *   (eval.py:182-197).  scale_shift [B][2] fp32 from a 2x2 solve in fp64; a constant prediction p gets lstsq's
+ *   minimum-norm solution (p, 1) * mean(g) / (p^2 + 1), an empty mask (0, 0).
+ * b200_eval_depth_metrics: eval.py:173-220 after the solve, one pass over pred / gt / mask [B][HW] (mask NULL = the
+ *   metrics' valid_mask=None):  p = pred * s + t (two fp32 roundings, scale_shift NULL = no alignment); disparity:
+ *   p = 1 / max(p, 1e-3); clip: p = max(clip(p, min_depth, max_depth), 1e-6).  aligned (nullable) [B][HW] receives p.
+ *   out (nullable: then gt may be NULL and only `aligned` is written) fp32[10] = abs_relative_difference,
+ *   squared_relative_difference, rmse_linear, rmse_log, log10, delta1_acc, delta2_acc, delta3_acc, i_rmse, silog_rmse
+ *   of Marigold/src/util/metric.py with its batch semantics: per-sample means averaged over B, log10 pooled over the
+ *   batch's pixels, silog with the batch mean inside the sqrt.  Per-pixel terms fp32, sums fp64; an empty mask gives NaN.
+ * b200_eval_normal_error: DSINE/utils/utils.py:150-159 and the accumulation of DSINE/projects/dsine/test.py:100-115.
+ *   pred / gt [B][3][H][W] read with element strides {b, c, h, w} (host arrays), so [3,H,W] and [H,W,3] maps are read in
+ *   place; mask [B][H][W] (NULL = every pixel).  Angle acos(clamp(x.y / (max(|x|,1e-8) max(|y|,1e-8)), -1, 1)) * 180 / pi
+ *   in degrees (torch.cosine_similarity), the cosine in fp64 rounded once to fp32.  err_map (nullable) [B][H][W].  buf (nullable): the
+ *   masked angles are appended, compacted in no particular order, at buf[*buf_len ...] (*buf_len advanced; writes past
+ *   buf_capacity are dropped).  sums / counts (nullable together): sums[2] += (sum e, sum e^2), counts[6] += (n, #e < 5,
+ *   7.5, 11.25, 22.5, 30) over the masked pixels.
+ * b200_eval_kth_smallest: exact k-th smallest (0-based) of x[0 .. *n) (*n read on the device; n_max >= *n sizes the
+ *   grid) by a radix select on the fp32 bit patterns: finite, non-negative values (-0 counts as +0).  k < 0 = the
+ *   median: k = (n - 1) / 2.  out[0] = k-th, out[1] = (k+1)-th (the k-th when k is the last), out[2] = the median as
+ *   np.median gives it on a float32 array ((out[0] + out[1]) / 2 in fp32 for an even count) for k < 0, out[0] else;
+ *   NaN when k >= n.  ws: unsigned long long[B200_EVAL_KTH_WS_WORDS]. */
+#define B200_EVAL_MAX_BLOCKS 512
+#define B200_EVAL_KTH_WS_WORDS 261
+int b200_eval_align_depth(const float* gt, const float* pred, const unsigned char* mask, int B, int H, int W, int OW,
+                          float col_scale, int disparity, double* ws, float* scale_shift, void* stream);
+int b200_eval_depth_metrics(const float* pred, const float* gt, const unsigned char* mask, int B, long long HW,
+                            const float* scale_shift, int disparity, int clip, float min_depth, float max_depth,
+                            float* aligned, double* ws, float* out, void* stream);
+int b200_eval_normal_error(const float* pred, const long long* pred_strides, const float* gt,
+                           const long long* gt_strides, const unsigned char* mask, int B, int H, int W, float* err_map,
+                           float* buf, long long buf_capacity, unsigned long long* buf_len, double* ws, double* sums,
+                           long long* counts, void* stream);
+int b200_eval_kth_smallest(const float* x, const unsigned long long* n, long long n_max, long long k,
+                           unsigned long long* ws, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
