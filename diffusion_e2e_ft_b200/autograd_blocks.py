@@ -244,7 +244,7 @@ class _TransformerFn(torch.autograd.Function):
         x, mr0, hn, h0, n1, qkv, o, h1, n2, q2, c2d, kv, o2, h2, n3, gg, h16 = saved
         pk, bp = m._packed(), blk._packed()
         B, H, W, C = x.shape
-        L, heads, scale = H * W, blk.heads, 64 ** -0.5
+        L, heads, scale = H * W, blk.heads, blk.head_dim ** -0.5
         S = kv.shape[1]
         train = _any(ctx, 5)
         proj = blk.ff.net[0].proj
@@ -303,6 +303,8 @@ class _TransformerFn(torch.autograd.Function):
                                                        False, [dout.view(B, H, W, C)], F32)
         order = ("gnw", "gnb", "wi", "bi", "wo", "bo", "ln1w", "ln1b", "wq1", "wk1", "wv1", "wo1", "bo1",
                  "ln2w", "ln2b", "wq2", "wk2", "wv2", "wo2", "bo2", "ln3w", "ln3b", "wp", "bp", "wf", "bf")
+        if train:                       # 1x1-conv projections: the [C, C] GEMM gradient in the [C, C, 1, 1] layout
+            g["wi"], g["wo"] = g["wi"].view(m.proj_in.weight.shape), g["wo"].view(m.proj_out.weight.shape)
         grads = [g.get(k) if train else None for k in order]
         return (None, None, None, dx, None, *grads)
 

@@ -193,8 +193,8 @@ def conv_dgrad(dy, w, cin, kind="s1", out_dtype=F32, add=None, packed=None, in_h
 
 # --------------------------------------------------------------------------------------------- attention
 def attention_bwd(q, k, v, do, heads, scale, outs=None):
-    """Backward of softmax(scale * q k^T) v per head (head dim 64).  q/do [B,T,heads*64], k/v [B,Tk,heads*64] fp16
-    views (last dim contiguous).  Returns fp16 (dq, dk, dv) — written into `outs` (row-strided views, e.g. the three
+    """Backward of softmax(scale * q k^T) v per head of width D = C / heads in ops.HEAD_DIMS.  q/do [B,T,C],
+    k/v [B,Tk,C] fp16 views (last dim contiguous).  Returns fp16 (dq, dk, dv) — written into `outs` (row-strided views, e.g. the three
     column blocks of a fused d(qkv) buffer) when given.
 
     Round 2: no fp32 score matrices and no softmax passes.  The flash kernel is re-run for (O, log-sum-exp); then per
@@ -207,7 +207,8 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
     Still materialises P and dS ([heads, T, Tk] fp16 per image): a fused flash backward would remove those too."""
     B, T, C = q.shape
     Tk = k.shape[1]
-    assert C == heads * 64
+    D = C // heads
+    assert C == heads * D and D in ops.HEAD_DIMS, (C, heads)
     Tkp = ops._ru8(Tk)
     dev = q.device
     if outs is not None:
@@ -229,11 +230,11 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
             dv[b, 0].copy_(ops.cast_f16(ops.col_sum(do[b])))
         return dq, dk, dv
 
-    def heads_view(t2d):                      # [L, heads*64] -> [heads, L, 64] strided view
-        return t2d.unflatten(-1, (heads, 64)).permute(1, 0, 2)
+    def heads_view(t2d):                      # [L, heads*D] -> [heads, L, D] strided view
+        return t2d.unflatten(-1, (heads, D)).permute(1, 0, 2)
 
-    o, lse = ops.attention_d64(q, k, v, heads, scale, want_lse=True)          # [B,T,C], [B,heads,T] (log2 domain)
-    delta = ops.rowdot_heads(do, o, heads)                                   # [B,heads,T]
+    o, lse = ops.attention(q, k, v, heads, scale, want_lse=True)             # [B,T,C], [B,heads,T] (log2 domain)
+    delta = ops.rowdot_heads_d(do, o, heads, D)                              # [B,heads,T]
     neg_lse = _scaled(lse, -1.0)
     neg_delta = _scaled(delta, -float(scale))
     c = float(scale) * 1.4426950408889634
@@ -244,7 +245,7 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
         ds = torch.empty((heads, T, Tkp), dtype=F16, device=dev)
         ops.linear(doh, vh, bias=neg_delta[b], bias_row=True, alpha=float(scale), residual=p[:, :, :Tk], res_mul=True,
                    out=ds[:, :, :Tk])
-        # dQ[h] = dS[h] @ K[h]            (K [Tk, 64] = [contraction, columns])
+        # dQ[h] = dS[h] @ K[h]            (K [Tk, D] = [contraction, columns])
         ops.linear(ds[:, :, :Tk], kh, out=heads_view(dq[b]), w_t=True)
         # dK[h] = dS[h]^T @ Q[h], dV[h] = P[h]^T @ dO[h]   (contraction over the T query rows of both operands)
         ops.linear(ds[:, :, :Tk], qh, out=heads_view(dk[b]), a_t=True, w_t=True)

@@ -58,10 +58,8 @@ class PretrainedMixin:
         for k, v in known.items():
             if isinstance(cls._config_defaults[k], tuple) and isinstance(v, list):
                 known[k] = tuple(v)
-        # diffusers stores a scalar attention_head_dim for SD-1 style models; the engine wants one entry per block
-        if "attention_head_dim" in known and not isinstance(known["attention_head_dim"], tuple):
-            n = len(known.get("block_out_channels", cls._config_defaults.get("block_out_channels", ())))
-            known["attention_head_dim"] = (known["attention_head_dim"],) * n
+        # a scalar attention_head_dim (diffusers' SD-1 configs) stays a scalar: the model expands it per block and
+        # save_pretrained writes it back as it was read
         extra = {k: v for k, v in raw.items() if k not in cls._config_defaults and k != "_class_name"}
         return known, extra
 

@@ -1,31 +1,55 @@
-// Flash attention on sm_90a: softmax(Q K^T * scale) V, no mask.  attention_d64_kernel (UNet heads, head_dim 64) first,
-// attention_d512_kernel (the single-head VAE mid-block) below.
+// Flash attention on sm_90a: softmax(Q K^T * scale) V, no mask.  attention_kernel<D> (UNet heads of width D in
+// {40, 64, 80, 160}) first, attention_d512_kernel (the single-head VAE mid-block) below.
 //
-// Warp-specialised, 192 query rows per CTA: warp 12 = TMA producer (the three Q tiles once, K/V tiles through a
-// 3-stage smem ring), warps 0..11 = three consumer warpgroups, each owning 64 query rows with S, P and O in registers.
-// Per key tile j and warpgroup w:
-//   S = Q_w K_j^T        wgmma m64n128k16 x 4, both operands from smem (K-major)  -> 64 fp32 registers per thread
+// Warp-specialised, WG x 64 query rows per CTA: warp 4 WG = TMA producer (the Q tiles once, K/V tiles through a
+// STAGES-deep smem ring), warps 0 .. 4 WG - 1 = WG consumer warpgroups, each owning 64 query rows with S, P and O in
+// registers.  Per key tile j (BK keys) and warpgroup w:
+//   S = Q_w K_j^T        wgmma m64n<BK>k16 x ceil(D/16), both operands from smem (K-major)  -> BK/2 fp32 registers
 //   m, l, O *= alpha     online softmax; a row lives in the 4 lanes of a quad, so the row max / sum take 2 shuffles
 //   P = exp2(S*c - m*c)  fp16, repacked in registers straight into the A-operand fragment layout
-//   O += P V_j           wgmma m64n64k16 x 8, A = P from registers, V consumed MN-major from its [keys x d] TMA tile
-// The three warpgroups run independently; while one exponentiates, the tensor core serves the others.
+//   O += P V_j           wgmma m64n<D>k16 x BK/16, A = P from registers, V consumed MN-major from its [keys x d] tile
+// The warpgroups run independently; while one exponentiates, the tensor core serves the others.
 // Joint attention (GeoWizard): kv_segments = 2 walks the K/V tiles of batch b%(B/2) then
 // b%(B/2)+B/2 — the concatenated K/V of attention.py:482-491 is never materialised.
+//
+// Operand tiles: Q / K / V are read in place through a 4-d tensor map {D, heads, L, B} whose innermost dimension is
+// one head, in 64-column SWIZZLE_128B boxes: ceil(D/64) atoms per row, the columns past D zero-filled by TMA (a head
+// slice of width 40 / 80 / 160 is 80 / 160 / 320 bytes, so the next head is never read).  The zero columns add
+// nothing to Q K^T; the P V product is N = D wide and never reads them.
+// Tile shape per D (the O accumulator is D/2 fp32 registers per thread, a K or V tile BK x ceil(D/64) x 128 bytes).
+// A 416-thread CTA (13 warps, allocated as 16) may use 128 registers per thread, a 288-thread one (9 warps, as 12) 168:
+//   D = 40, 64   3 warpgroups, 128-key tiles, 3 stages   (Q 24 KB + K/V 96 KB; S 64 + P 32 + O <= 32 registers)
+//   D = 80       3 warpgroups,  64-key tiles, 3 stages   (Q 48 KB + K/V 96 KB; 128-key tiles spill at 128 registers)
+//   D = 160      2 warpgroups,  64-key tiles, 3 stages   (Q 48 KB + K/V 144 KB; O 80 + S 32 + P 16 registers)
 #include "common.cuh"
 #include "wgmma.cuh"
 #include "../../include/b200_e2eft.h"
 
 namespace b200 {
 
-constexpr int kAttWG = 3;                        // consumer warpgroups (query tiles) per CTA
-constexpr int kAttThreads = 128 * kAttWG + 32;   // + the TMA producer warp
 constexpr int kBq = 64;                          // query rows per warpgroup
-constexpr int kBk = 128;                         // keys per tile
-constexpr int kD = 64;
-constexpr int kKvStages = 3;
-constexpr int kQBytes = kBq * kD * 2;            // 8 KB
-constexpr int kKvBytes = kBk * kD * 2;           // 16 KB (K or V tile)
-constexpr int kAttSmem = kAttWG * kQBytes + kKvStages * 2 * kKvBytes + 1024 + 1024;
+
+template <int D> struct AttCfg;
+template <> struct AttCfg<40> { static constexpr int kWG = 3, kBk = 128, kStages = 3; };
+template <> struct AttCfg<64> { static constexpr int kWG = 3, kBk = 128, kStages = 3; };
+template <> struct AttCfg<80> { static constexpr int kWG = 3, kBk = 64, kStages = 3; };
+template <> struct AttCfg<160> { static constexpr int kWG = 2, kBk = 64, kStages = 3; };
+
+template <int D>
+struct AttShape : AttCfg<D> {
+  using AttCfg<D>::kWG;
+  using AttCfg<D>::kBk;
+  using AttCfg<D>::kStages;
+  static constexpr int kAtoms = (D + 63) / 64;               // 64-column SWIZZLE_128B atoms per row
+  static constexpr int kKSteps = (D + 15) / 16;              // k16 steps of Q K^T
+  static constexpr int kThreads = 128 * kWG + 32;            // + the TMA producer warp
+  static constexpr int kQAtom = kBq * 128;                   // one 64-row atom of a Q tile
+  static constexpr int kKvAtom = kBk * 128;                  // one BK-row atom of a K or V tile
+  static constexpr int kQBytes = kAtoms * kQAtom;
+  static constexpr int kKvBytes = kAtoms * kKvAtom;
+  static constexpr int kSmem = kWG * kQBytes + kStages * 2 * kKvBytes + 1024 + 1024;
+  static_assert(kSmem <= 227 * 1024, "attention shared memory");
+};
 
 struct AttParams {
   int B, heads, Lq, Lk, kv_segments;
@@ -46,51 +70,70 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return r;
 }
 
-__global__ void __launch_bounds__(kAttThreads, 1)
-attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const AttParams p) {
+template <int BK>
+__device__ __forceinline__ void wgmma_qk(float* s, uint64_t da, uint64_t db, int scale_d) {
+  if constexpr (BK == 128) wgmma_m64n128<0, 0>(s, da, db, scale_d);
+  else wgmma_m64n64<0, 0>(s, da, db, scale_d);
+}
+
+template <int D>
+__device__ __forceinline__ void wgmma_pv(float* o, const uint32_t (&a)[4], uint64_t db) {
+  if constexpr (D == 40) wgmma_m64n40_rs_bmn(o, a, db);
+  else if constexpr (D == 64) wgmma_m64n64_rs_bmn(o, a, db);
+  else if constexpr (D == 80) wgmma_m64n80_rs_bmn(o, a, db);
+  else wgmma_m64n160_rs_bmn(o, a, db);
+}
+
+template <int D>
+__global__ void __launch_bounds__(AttShape<D>::kThreads, 1)
+attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                 const __grid_constant__ CUtensorMap tmV, const AttParams p) {
+  using S_ = AttShape<D>;
+  constexpr int kWG = S_::kWG, kBk = S_::kBk, kStages = S_::kStages, kAtoms = S_::kAtoms;
+  constexpr int kQBytes = S_::kQBytes, kKvBytes = S_::kKvBytes;
   // 1024-byte alignment (SWIZZLE_128B atoms) by pointer arithmetic on the __shared__ array itself, so
   // the compiler keeps the shared address space (LDS/STS, no aliasing with global stores)
   extern __shared__ __align__(16) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* sQ = smem;                                   // [kAttWG][8 KB]
-  uint8_t* sK = sQ + kAttWG * kQBytes;                  // [stages][16 KB]
-  uint8_t* sV = sK + kKvStages * kKvBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kKvStages * kKvBytes);
+  uint8_t* sQ = smem;                                   // [kWG][kAtoms][64 rows x 128 B]
+  uint8_t* sK = sQ + kWG * kQBytes;                     // [stages][kAtoms][kBk rows x 128 B]
+  uint8_t* sV = sK + kStages * kKvBytes;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kStages * kKvBytes);
   uint64_t* q_full = bars;
   uint64_t* k_full = bars + 1;
-  uint64_t* v_full = k_full + kKvStages;
-  uint64_t* kv_empty = v_full + kKvStages;
+  uint64_t* v_full = k_full + kStages;
+  uint64_t* kv_empty = v_full + kStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int q0 = blockIdx.x * (kAttWG * kBq);
+  const int q0 = blockIdx.x * (kWG * kBq);
   const int h = blockIdx.y;
   const int b = blockIdx.z;
   const int tiles_per_seg = (p.Lk + kBk - 1) / kBk;
   const int n_tiles = tiles_per_seg * p.kv_segments;
   const int half_b = p.kv_segments == 2 ? p.B / 2 : 0;
 
-  if (warp == 4 * kAttWG && lane == 0) {
+  if (warp == 4 * kWG && lane == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
-    for (int i = 0; i < kKvStages; ++i) {
+    for (int i = 0; i < kStages; ++i) {
       mbar_init(&k_full[i], 1);
       mbar_init(&v_full[i], 1);
-      mbar_init(&kv_empty[i], 128 * kAttWG);
+      mbar_init(&kv_empty[i], 128 * kWG);
     }
     fence_barrier_init();
   }
   __syncthreads();
 
-  if (warp == 4 * kAttWG) {
+  if (warp == 4 * kWG) {
     // ===================================================================== TMA producer
     if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, kAttWG * kQBytes);
-      for (int w = 0; w < kAttWG; ++w)
-        tma_load_3d(&tmQ, q_full, sQ + w * kQBytes, h * kD, q0 + w * kBq, b, kEvictFirst);
+      mbar_arrive_expect_tx(q_full, kWG * kQBytes);
+      for (int w = 0; w < kWG; ++w)
+        for (int a = 0; a < kAtoms; ++a)
+          tma_load_4d(&tmQ, q_full, sQ + w * kQBytes + a * S_::kQAtom, 64 * a, h, q0 + w * kBq, b, kEvictFirst);
       int stage = 0;
       uint32_t phase = 0;
       for (int seg = 0; seg < p.kv_segments; ++seg) {
@@ -98,10 +141,14 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         for (int j = 0; j < tiles_per_seg; ++j) {
           mbar_wait(&kv_empty[stage], phase ^ 1);
           mbar_arrive_expect_tx(&k_full[stage], kKvBytes);
-          tma_load_3d(&tmK, &k_full[stage], sK + stage * kKvBytes, h * kD, j * kBk, kb, kEvictLast);
+          for (int a = 0; a < kAtoms; ++a)
+            tma_load_4d(&tmK, &k_full[stage], sK + stage * kKvBytes + a * S_::kKvAtom, 64 * a, h, j * kBk, kb,
+                        kEvictLast);
           mbar_arrive_expect_tx(&v_full[stage], kKvBytes);
-          tma_load_3d(&tmV, &v_full[stage], sV + stage * kKvBytes, h * kD, j * kBk, kb, kEvictLast);
-          if (++stage == kKvStages) { stage = 0; phase ^= 1; }
+          for (int a = 0; a < kAtoms; ++a)
+            tma_load_4d(&tmV, &v_full[stage], sV + stage * kKvBytes + a * S_::kKvAtom, 64 * a, h, j * kBk, kb,
+                        kEvictLast);
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
     }
@@ -113,17 +160,17 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
   // 8 i + 2 (lane % 4) + {0, 1}: s[4i], s[4i+1] for row r0, s[4i+2], s[4i+3] for row r0 + 8
   const int r0 = (warp & 3) * 16 + (lane >> 2);
   const int cq = 2 * (lane & 3);
-  float o[kD / 2];
+  float o[D / 2];
 #pragma unroll
-  for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+  for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   const float c = p.scale_log2;
   const uint64_t qdesc = make_desc_sw128(smem_u32(sQ + w * kQBytes), 16, 1024);
   mbar_wait(q_full, 0);
 
   for (int j = 0; j < n_tiles; ++j) {
-    const int st = j % kKvStages;
-    const uint32_t ph = (j / kKvStages) & 1;
+    const int st = j % kStages;
+    const uint32_t ph = (j / kStages) & 1;
     const int jj = j % tiles_per_seg;
     const int valid = min(kBk, p.Lk - jj * kBk);
     float s[kBk / 2];
@@ -132,7 +179,9 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       const uint64_t kdesc = make_desc_sw128(smem_u32(sK + st * kKvBytes), 16, 1024);
       wgmma_fence();
 #pragma unroll
-      for (int k = 0; k < kD / 16; ++k) wgmma_m64n128<0, 0>(s, qdesc + 2 * k, kdesc + 2 * k, k != 0);
+      for (int k = 0; k < S_::kKSteps; ++k)        // k-step k: columns 16 (k % 4) .. of atom k / 4 (+32 B per step)
+        wgmma_qk<kBk>(s, qdesc + (k / 4) * (S_::kQAtom >> 4) + 2 * (k % 4),
+                      kdesc + (k / 4) * (S_::kKvAtom >> 4) + 2 * (k % 4), k != 0);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_operands<kBk / 2>(s);
@@ -182,7 +231,7 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
     for (int r = 0; r < 2; ++r) l[r] = fmaf(l[r], alpha[r], rs[r]);
 #pragma unroll
-    for (int i = 0; i < kD / 8; ++i) {
+    for (int i = 0; i < D / 8; ++i) {
       o[4 * i] *= alpha[0];
       o[4 * i + 1] *= alpha[0];
       o[4 * i + 2] *= alpha[1];
@@ -191,14 +240,14 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     mbar_wait(&v_full[st], ph);
     {
       const uint32_t vbase = smem_u32(sV + st * kKvBytes);
-      wgmma_fence_operands<kD / 2>(o);
+      wgmma_fence_operands<D / 2>(o);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kBk / 16; ++kk)       // B = V[16 kk .. 16 kk + 15, :]: MN-major, 2 groups of 8 key rows
-        wgmma_m64n64_rs_bmn(o, pa[kk], make_desc_sw128(vbase + kk * 2048, 8192, 1024));
+        wgmma_pv<D>(o, pa[kk], make_desc_sw128(vbase + kk * 2048, S_::kKvAtom, 1024));   // atoms kKvAtom apart
       wgmma_commit();
       wgmma_wait<0>();
-      wgmma_fence_operands<kD / 2>(o);
+      wgmma_fence_operands<D / 2>(o);
     }
     mbar_arrive(&kv_empty[st]);                      // this warpgroup is done with K_j / V_j
   }
@@ -214,9 +263,9 @@ attention_d64_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     if (p.lse != nullptr && (lane & 3) == 0)       // P_ij = exp2(S_ij * c - lse): what the backward pass recomputes P from
       p.lse[((long long)b * p.heads + h) * p.Lq + qrow] = fmaf(m[r], c, log2f(l[r]));
     const float inv = 1.0f / l[r];
-    __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + h * kD + cq;
+    __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + h * D + cq;
 #pragma unroll
-    for (int i = 0; i < kD / 8; ++i)
+    for (int i = 0; i < D / 8; ++i)
       *reinterpret_cast<uint32_t*>(dst + 8 * i) = pack_half2(o[4 * i + 2 * r] * inv, o[4 * i + 2 * r + 1] * inv);
   }
 }
@@ -439,57 +488,85 @@ attention_d512_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
 using namespace b200;
 
 
-extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls, const void* k,
-                                  long long k_bs, long long k_ls, const void* v, long long v_bs,
-                                  long long v_ls, void* out, long long o_bs, long long o_ls, int B,
-                                  int heads, int Lq, int Lk, int kv_segments, float scale, float* lse,
-                                  void* stream) {
-  B200_CHECK_ARG(q && k && v && out, "b200_attention_d64: null pointer");
-  B200_CHECK_ARG(B > 0 && heads > 0 && Lq > 0 && Lk > 0, "b200_attention_d64: bad shape");
-  B200_CHECK_ARG(kv_segments == 1 || (kv_segments == 2 && B % 2 == 0), "b200_attention_d64: kv_segments=%d B=%d", kv_segments, B);
-  B200_CHECK_ARG(q_ls % 8 == 0 && k_ls % 8 == 0 && v_ls % 8 == 0 && o_ls % 8 == 0 && q_bs % 8 == 0 &&
-                     k_bs % 8 == 0 && v_bs % 8 == 0 && o_bs % 8 == 0,
-                 "b200_attention_d64: strides must be multiples of 8 elements");
-  B200_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) == 0,
-                 "b200_attention_d64: pointers must be 16-byte aligned");
+namespace {
+
+template <int D>
+int launch_attention(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs, long long k_ls,
+                     const void* v, long long v_bs, long long v_ls, const AttParams& p, void* stream) {
+  using S_ = AttShape<D>;
+  // {D, heads, L, B}: one head is the innermost dimension, so a 64-column box past D reads zeros, not the next head
   CUtensorMap tq, tk, tv;
-  const uint32_t box[3] = {kD, kBq, 1};
-  const uint32_t kv_box[3] = {kD, kBk, 1};
+  const uint32_t box[4] = {64, 1, kBq, 1};
+  const uint32_t kv_box[4] = {64, 1, S_::kBk, 1};
   {
-    uint64_t dims[3] = {(uint64_t)heads * kD, (uint64_t)Lq, (uint64_t)B};
-    uint64_t str[2] = {(uint64_t)q_ls * 2, (uint64_t)q_bs * 2};
-    int r = encode_tmap(&tq, q, 3, dims, str, box, nullptr);
+    uint64_t dims[4] = {(uint64_t)D, (uint64_t)p.heads, (uint64_t)p.Lq, (uint64_t)p.B};
+    uint64_t str[3] = {(uint64_t)D * 2, (uint64_t)q_ls * 2, (uint64_t)q_bs * 2};
+    int r = encode_tmap(&tq, q, 4, dims, str, box, nullptr);
     if (r) return r;
   }
   {
-    uint64_t dims[3] = {(uint64_t)heads * kD, (uint64_t)Lk, (uint64_t)B};
-    uint64_t str[2] = {(uint64_t)k_ls * 2, (uint64_t)k_bs * 2};
-    int r = encode_tmap(&tk, k, 3, dims, str, kv_box, nullptr);
+    uint64_t dims[4] = {(uint64_t)D, (uint64_t)p.heads, (uint64_t)p.Lk, (uint64_t)p.B};
+    uint64_t str[3] = {(uint64_t)D * 2, (uint64_t)k_ls * 2, (uint64_t)k_bs * 2};
+    int r = encode_tmap(&tk, k, 4, dims, str, kv_box, nullptr);
     if (r) return r;
-    uint64_t strv[2] = {(uint64_t)v_ls * 2, (uint64_t)v_bs * 2};
-    r = encode_tmap(&tv, v, 3, dims, strv, kv_box, nullptr);
+    uint64_t strv[3] = {(uint64_t)D * 2, (uint64_t)v_ls * 2, (uint64_t)v_bs * 2};
+    r = encode_tmap(&tv, v, 4, dims, strv, kv_box, nullptr);
     if (r) return r;
   }
   static bool configured_dev[kMaxDevices] = {false};      // per device: function attributes live in the context
   const int dev_ = current_device();
   bool& configured = configured_dev[dev_ < 0 ? 0 : dev_];
   if (!configured || dev_ < 0) {
-    cudaError_t e = cudaFuncSetAttribute(attention_d64_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttSmem);
+    cudaError_t e = cudaFuncSetAttribute(attention_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, S_::kSmem);
     if (e != cudaSuccess) {
-      set_last_error("cudaFuncSetAttribute(attention smem=%d): %s", kAttSmem, cudaGetErrorString(e));
+      set_last_error("cudaFuncSetAttribute(attention head_dim=%d smem=%d): %s", D, S_::kSmem, cudaGetErrorString(e));
       return (int)e;
     }
     configured = true;
   }
+  dim3 grid((p.Lq + S_::kWG * kBq - 1) / (S_::kWG * kBq), p.heads, p.B);
+  attention_kernel<D><<<grid, S_::kThreads, S_::kSmem, (cudaStream_t)stream>>>(tq, tk, tv, p);
+  B200_CHECK_LAUNCH("attention_kernel");
+  return 0;
+}
+
+}  // namespace
+
+extern "C" int b200_attention(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs,
+                              long long k_ls, const void* v, long long v_bs, long long v_ls, void* out, long long o_bs,
+                              long long o_ls, int B, int heads, int head_dim, int Lq, int Lk, int kv_segments,
+                              float scale, float* lse, void* stream) {
+  B200_CHECK_ARG(head_dim == 40 || head_dim == 64 || head_dim == 80 || head_dim == 160,
+                 "b200_attention: head_dim=%d is not one of 40, 64, 80, 160", head_dim);
+  B200_CHECK_ARG(q && k && v && out, "b200_attention: null pointer");
+  B200_CHECK_ARG(B > 0 && B <= 65535 && heads > 0 && heads <= 65535 && Lq > 0 && Lk > 0,
+                 "b200_attention: bad shape B=%d heads=%d Lq=%d Lk=%d", B, heads, Lq, Lk);
+  B200_CHECK_ARG(kv_segments == 1 || (kv_segments == 2 && B % 2 == 0), "b200_attention: kv_segments=%d B=%d", kv_segments, B);
+  B200_CHECK_ARG(q_ls % 8 == 0 && k_ls % 8 == 0 && v_ls % 8 == 0 && o_ls % 8 == 0 && q_bs % 8 == 0 &&
+                     k_bs % 8 == 0 && v_bs % 8 == 0 && o_bs % 8 == 0,
+                 "b200_attention: strides must be multiples of 8 elements");
+  B200_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) == 0,
+                 "b200_attention: pointers must be 16-byte aligned");
   AttParams p;
   p.B = B; p.heads = heads; p.Lq = Lq; p.Lk = Lk; p.kv_segments = kv_segments;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = (__half*)out; p.o_bs = o_bs; p.o_ls = o_ls;
   p.lse = lse;
-  dim3 grid((Lq + kAttWG * kBq - 1) / (kAttWG * kBq), heads, B);
-  attention_d64_kernel<<<grid, kAttThreads, kAttSmem, (cudaStream_t)stream>>>(tq, tk, tv, p);
-  B200_CHECK_LAUNCH("attention_d64_kernel");
-  return 0;
+  switch (head_dim) {
+    case 40: return launch_attention<40>(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, p, stream);
+    case 64: return launch_attention<64>(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, p, stream);
+    case 80: return launch_attention<80>(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, p, stream);
+    default: return launch_attention<160>(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, p, stream);
+  }
+}
+
+extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls, const void* k,
+                                  long long k_bs, long long k_ls, const void* v, long long v_bs,
+                                  long long v_ls, void* out, long long o_bs, long long o_ls, int B,
+                                  int heads, int Lq, int Lk, int kv_segments, float scale, float* lse,
+                                  void* stream) {
+  return b200_attention(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, out, o_bs, o_ls, B, heads, 64, Lq, Lk,
+                        kv_segments, scale, lse, stream);
 }
 
 extern "C" int b200_attention_d512(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs,

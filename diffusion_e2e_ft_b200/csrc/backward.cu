@@ -103,8 +103,9 @@ __global__ void gather_planar_kernel(const T* __restrict__ x, long long ldx, int
 }
 
 // ------------------------------------------------------------------------------------------------ rowdot
-// delta[b][h][t] = sum_{d < 64} a[b][t][h*64 + d] * c[b][t][h*64 + d]   (fp16 in, fp32 accumulate / out).
-// One warp per (t, h): 64 elements = one __half2 per lane.
+// delta[b][h][t] = sum_{d < D} a[b][t][h*D + d] * c[b][t][h*D + d]   (fp16 in, fp32 accumulate / out).
+// One warp per (t, h): lane l reads the __half2 at d = 64 j + 2 l of each 64-column chunk j that reaches it.
+template <int D>
 __global__ void rowdot_heads_kernel(const __half* __restrict__ a, long long a_bs, long long a_ls,
                                     const __half* __restrict__ c, long long c_bs, long long c_ls, int L, int heads,
                                     float* __restrict__ out) {
@@ -112,10 +113,19 @@ __global__ void rowdot_heads_kernel(const __half* __restrict__ a, long long a_bs
   const int t = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (t >= L) return;
   const int lane = threadIdx.x & 31;
-  const __half2 x = *reinterpret_cast<const __half2*>(a + (long long)b * a_bs + (long long)t * a_ls + h * 64 + 2 * lane);
-  const __half2 y = *reinterpret_cast<const __half2*>(c + (long long)b * c_bs + (long long)t * c_ls + h * 64 + 2 * lane);
-  const float2 xf = __half22float2(x), yf = __half22float2(y);
-  float s = fmaf(xf.x, yf.x, xf.y * yf.y);
+  const __half* ar = a + (long long)b * a_bs + (long long)t * a_ls + h * D;
+  const __half* cr = c + (long long)b * c_bs + (long long)t * c_ls + h * D;
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < (D + 63) / 64; ++j) {
+    const int d = 64 * j + 2 * lane;
+    if (d < D) {
+      const float2 xf = __half22float2(*reinterpret_cast<const __half2*>(ar + d));
+      const float2 yf = __half22float2(*reinterpret_cast<const __half2*>(cr + d));
+      const float v = fmaf(xf.x, yf.x, xf.y * yf.y);
+      s = j == 0 ? v : s + v;
+    }
+  }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
   if (lane == 0) out[((long long)b * heads + h) * L + t] = s;
@@ -639,16 +649,29 @@ extern "C" int b200_gather_planar(const void* x, int in_f32, long long ldx, int 
   return 0;
 }
 
-extern "C" int b200_rowdot_heads(const void* a, long long a_bs, long long a_ls, const void* c, long long c_bs,
-                                 long long c_ls, int B, int L, int heads, float* out, void* stream) {
+extern "C" int b200_rowdot_heads_d(const void* a, long long a_bs, long long a_ls, const void* c, long long c_bs,
+                                   long long c_ls, int B, int L, int heads, int head_dim, float* out, void* stream) {
+  B200_CHECK_ARG(head_dim == 40 || head_dim == 64 || head_dim == 80 || head_dim == 160,
+                 "b200_rowdot_heads_d: head_dim=%d is not one of 40, 64, 80, 160", head_dim);
   B200_CHECK_ARG(a && c && out && B > 0 && L > 0 && heads > 0, "b200_rowdot_heads: bad arguments");
   B200_CHECK_ARG(a_ls % 2 == 0 && c_ls % 2 == 0 && a_bs % 2 == 0 && c_bs % 2 == 0 &&
                      (((uintptr_t)a | (uintptr_t)c) & 3) == 0, "b200_rowdot_heads: 4-byte alignment");
   dim3 grid((L + 7) / 8, heads, B);
-  rowdot_heads_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)a, a_bs, a_ls, (const __half*)c, c_bs, c_ls, L,
-                                                              heads, out);
+  const cudaStream_t st = (cudaStream_t)stream;
+  const __half *ah = (const __half*)a, *ch = (const __half*)c;
+  switch (head_dim) {
+    case 40: rowdot_heads_kernel<40><<<grid, 256, 0, st>>>(ah, a_bs, a_ls, ch, c_bs, c_ls, L, heads, out); break;
+    case 64: rowdot_heads_kernel<64><<<grid, 256, 0, st>>>(ah, a_bs, a_ls, ch, c_bs, c_ls, L, heads, out); break;
+    case 80: rowdot_heads_kernel<80><<<grid, 256, 0, st>>>(ah, a_bs, a_ls, ch, c_bs, c_ls, L, heads, out); break;
+    default: rowdot_heads_kernel<160><<<grid, 256, 0, st>>>(ah, a_bs, a_ls, ch, c_bs, c_ls, L, heads, out); break;
+  }
   B200_CHECK_LAUNCH("rowdot_heads_kernel");
   return 0;
+}
+
+extern "C" int b200_rowdot_heads(const void* a, long long a_bs, long long a_ls, const void* c, long long c_bs,
+                                 long long c_ls, int B, int L, int heads, float* out, void* stream) {
+  return b200_rowdot_heads_d(a, a_bs, a_ls, c, c_bs, c_ls, B, L, heads, 64, out, stream);
 }
 
 extern "C" int b200_col_sum(const void* x, int in_f32, long long rows, int C, long long ld, float* out, void* stream) {

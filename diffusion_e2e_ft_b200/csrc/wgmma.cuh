@@ -88,9 +88,27 @@ __device__ __forceinline__ void wgmma_m64n256(float* d, uint64_t da, uint64_t db
 }
 
 // A from registers (a[0..3] = the fp16 pairs of the accumulator-shaped 64 x 16 fragment), B MN-major
+__device__ __forceinline__ void wgmma_m64n40_rs_bmn(float* d, const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n40k16.f32.f16.f16 {" WG_R0 "," WG_R8 ",%16,%17,%18,%19}, {%20, %21, %22, %23}, %24, 1, 1, 1, 1;"
+               : WG_D(0), WG_D(8), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
 __device__ __forceinline__ void wgmma_m64n64_rs_bmn(float* d, const uint32_t (&a)[4], uint64_t db) {
   asm volatile("wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {" WG_R0 "," WG_R8 "," WG_R16 "," WG_R24 "}, {%32, %33, %34, %35}, %36, 1, 1, 1, 1;"
                : WG_D(0), WG_D(8), WG_D(16), WG_D(24)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
+__device__ __forceinline__ void wgmma_m64n80_rs_bmn(float* d, const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 {" WG_R0 "," WG_R8 "," WG_R16 "," WG_R24 "," WG_R32 "}, {%40, %41, %42, %43}, %44, 1, 1, 1, 1;"
+               : WG_D(0), WG_D(8), WG_D(16), WG_D(24), WG_D(32)
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
+__device__ __forceinline__ void wgmma_m64n160_rs_bmn(float* d, const uint32_t (&a)[4], uint64_t db) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n160k16.f32.f16.f16 {" WG_R0 "," WG_R8 "," WG_R16 "," WG_R24 "," WG_R32 "," WG_R40 "," WG_R48 "," WG_R56 "," WG_R64 "," WG_R72 "}, {%80, %81, %82, %83}, %84, 1, 1, 1, 1;"
+               : WG_D(0), WG_D(8), WG_D(16), WG_D(24), WG_D(32), WG_D(40), WG_D(48), WG_D(56), WG_D(64), WG_D(72)
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
 

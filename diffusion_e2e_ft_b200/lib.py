@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 13       # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 14       # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -38,10 +38,13 @@ _SIGS = {
     "b200_group_norm_apply_cs": (c_int, [_P, c_int, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, _P, _P, c_float,
                                          c_int, _P, _P, _P]),
     "b200_layer_norm": (c_int, [_P, c_int, _LL, c_int, _P, _P, c_float, _P, _P]),
+    "b200_attention": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_int,
+                               c_int, c_int, c_float, _P, _P]),
     "b200_attention_d64": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int,
                                    c_int, c_int, c_float, _P, _P]),
     "b200_attention_d512": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int,
                                     c_float, _P]),
+    "b200_rowdot_heads_d": (c_int, [_P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_int, _P, _P]),
     "b200_rowdot_heads": (c_int, [_P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, _P, _P]),
     "b200_softmax_rows": (c_int, [_P, _LL, _P, _LL, _LL, c_int, c_float, _P]),
     "b200_softmax_groups": (c_int, [_P, c_int, _LL, c_int, c_int, _P, c_int, _P]),

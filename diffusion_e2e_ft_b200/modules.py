@@ -261,8 +261,10 @@ class BasicTransformerBlock(nn.Module):
 
     def __init__(self, dim, heads, cross_dim, joint=False):
         super().__init__()
-        assert dim == heads * 64, "engine attention kernel is specialised for head_dim 64"
-        self.dim, self.heads, self.joint = dim, heads, joint
+        if dim % heads or dim // heads not in ops.HEAD_DIMS:
+            raise NotImplementedError(f"{dim} channels over {heads} heads is head width {dim / heads:g}; the engine's "
+                                      f"attention kernel supports head widths {ops.HEAD_DIMS}")
+        self.dim, self.heads, self.head_dim, self.joint = dim, heads, dim // heads, joint
         self.norm1 = nn.LayerNorm(dim, eps=1e-5)
         self.attn1 = Attention(dim)
         self.norm2 = nn.LayerNorm(dim, eps=1e-5)
@@ -287,16 +289,16 @@ class BasicTransformerBlock(nn.Module):
         params = [a2.to_q.weight, a2.to_k.weight, a2.to_v.weight, a2.to_out[0].weight, ctx1]
 
         def build():
-            C, heads = self.dim, self.heads
+            C, heads, D = self.dim, self.heads, self.head_dim
             S = ctx1.shape[0]
             J = heads * S
             Jp = (J + 7) // 8 * 8
             c = ctx1.detach().to(F32)
-            k = (c @ a2.to_k.weight.detach().to(F32).t()).view(S, heads, 64)           # [S, heads, 64]
-            v = (c @ a2.to_v.weight.detach().to(F32).t()).view(S, heads, 64)
-            wq = a2.to_q.weight.detach().to(F32).view(heads, 64, C)                    # rows of W_q per head
-            wo = a2.to_out[0].weight.detach().to(F32).view(C, heads, 64)               # columns of W_o per head
-            A = torch.einsum("shd,hdc->hsc", k, wq).reshape(J, C) * (64 ** -0.5)
+            k = (c @ a2.to_k.weight.detach().to(F32).t()).view(S, heads, D)            # [S, heads, D]
+            v = (c @ a2.to_v.weight.detach().to(F32).t()).view(S, heads, D)
+            wq = a2.to_q.weight.detach().to(F32).view(heads, D, C)                     # rows of W_q per head
+            wo = a2.to_out[0].weight.detach().to(F32).view(C, heads, D)                # columns of W_o per head
+            A = torch.einsum("shd,hdc->hsc", k, wq).reshape(J, C) * (D ** -0.5)
             VW = torch.einsum("shd,chd->hsc", v, wo).reshape(J, C)
             a16 = torch.zeros((Jp, C), dtype=F16, device=c.device)
             a16[:J] = A.to(F16)
@@ -326,10 +328,10 @@ class BasicTransformerBlock(nn.Module):
         assert not (save and const_ctx is not None), "the backward exists for the general cross-attention path only"
         pk = self._packed()
         C, heads = self.dim, self.heads
-        scale = 64 ** -0.5
+        scale = self.head_dim ** -0.5
         n1 = ops.layer_norm(h0, *pk["ln"][0])
         qkv = ops.linear(n1, pk["wqkv"]).view(B, L, 3 * C)
-        o = ops.attention_d64(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, scale,
+        o = ops.attention(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], heads, scale,
                               kv_segments=2 if self.joint else 1)
         h1 = ops.linear(o.view(B * L, C), pk["wo1"], pk["bo1"], residual=h0, out_dtype=sdt)
         n2 = ops.layer_norm(h1, *pk["ln"][1])
@@ -343,7 +345,7 @@ class BasicTransformerBlock(nn.Module):
             q2 = ops.linear(n2, pk["wq2"]).view(B, L, C)
             c2d = ctx16.reshape(B * S, -1)
             kv = ops.linear(c2d, pk["wkv2"]).view(B, S, 2 * C)
-            o2 = ops.attention_d64(q2, kv[..., :C], kv[..., C:], heads, scale)
+            o2 = ops.attention(q2, kv[..., :C], kv[..., C:], heads, scale)
             h2 = ops.linear(o2.view(B * L, C), pk["wo2"], pk["bo2"], residual=h1, out_dtype=sdt)
         saved = (n1, qkv, o, h1, n2, q2, c2d, kv, o2) if save else None
         del h1                          # without `save`, the feed-forward below runs with h1 already freed
@@ -357,24 +359,27 @@ class BasicTransformerBlock(nn.Module):
 
 
 class Transformer2DModel(nn.Module):
-    """GeoWizard/geowizard/models/transformer_2d.py:327-347,407-423 (continuous input, linear
-    projections): GN -> proj_in -> blocks -> proj_out -> + residual."""
+    """GeoWizard/geowizard/models/transformer_2d.py:327-347,407-423 (continuous input): GN -> proj_in -> blocks ->
+    proj_out -> + residual.  `use_linear_projection` (SD-2, Marigold) makes the projections nn.Linear; otherwise
+    (SD-1, GeoWizard) they are 1x1 nn.Conv2d with [C, C, 1, 1] weights (transformer_2d.py:152-155,214-217).  On NHWC
+    activations a 1x1 conv is the same [B*L, C] x [C, C]^T GEMM, so both run the same packed fp16 [C, C] weight."""
 
-    def __init__(self, dim, heads, cross_dim, groups=32, joint=False):
+    def __init__(self, dim, heads, cross_dim, groups=32, joint=False, use_linear_projection=True):
         super().__init__()
         self.dim, self.groups = dim, groups
         self.norm = nn.GroupNorm(groups, dim, eps=1e-6)
-        self.proj_in = nn.Linear(dim, dim)
+        self.proj_in = nn.Linear(dim, dim) if use_linear_projection else nn.Conv2d(dim, dim, 1)
         self.transformer_blocks = nn.ModuleList([BasicTransformerBlock(dim, heads, cross_dim, joint)])
-        self.proj_out = nn.Linear(dim, dim)
+        self.proj_out = nn.Linear(dim, dim) if use_linear_projection else nn.Conv2d(dim, dim, 1)
         self._pk = Packed()
 
     def _packed(self):
         own = [self.norm.weight, self.norm.bias, self.proj_in.weight, self.proj_in.bias,
                self.proj_out.weight, self.proj_out.bias]
+        C = self.dim
         return self._pk.get(own, lambda: dict(g=_f32(self.norm.weight), b=_f32(self.norm.bias),
-                                              wi=_f16(self.proj_in.weight), bi=_f32(self.proj_in.bias),
-                                              wo=_f16(self.proj_out.weight), bo=_f32(self.proj_out.bias)))
+                                              wi=_f16(self.proj_in.weight.reshape(C, C)), bi=_f32(self.proj_in.bias),
+                                              wo=_f16(self.proj_out.weight.reshape(C, C)), bo=_f32(self.proj_out.bias)))
 
     def run(self, x, ctx16, sdt=F32, f16_copy=False, const_ctx=None):
         return self.forward_saved(x, ctx16, sdt, f16_copy, const_ctx, save=False)[0]

@@ -316,27 +316,49 @@ def layer_norm(x, gamma, beta, eps=1e-5):
 
 
 # ------------------------------------------------------------------------------ attention
-@_timed("attention")
+HEAD_DIMS = (40, 64, 80, 160)          # head widths the flash kernel is instantiated for
+
+
+def attention(q, k, v, heads, scale, kv_segments=1, out=None, want_lse=False):
+    """Multi-head flash attention with head width D = C / heads, C = q.shape[-1], D in HEAD_DIMS.
+    q: [B,Lq,C] view, k/v: [B,Lk,C] views (fp16, last dim contiguous, e.g. column blocks of one fused QKV buffer)
+    -> [B,Lq,C].  `kv_segments` = 2: joint attention (batch b attends to the keys of b % (B/2) and b % (B/2) + B/2).
+    `want_lse`: also return the log2-domain log-sum-exp of the scaled scores, fp32 [B, heads, Lq]
+    (P_ij = exp2(scale * log2(e) * S_ij - lse_i)) for the backward pass.  Width 64 (SD-2) is `attention_d64`."""
+    C = q.shape[-1]
+    if C % heads or C // heads not in HEAD_DIMS:
+        raise ValueError(f"attention: {C} channels over {heads} heads is head width {C / heads:g}, "
+                         f"the kernel supports {HEAD_DIMS}")
+    if C // heads == 64:
+        return attention_d64(q, k, v, heads, scale, kv_segments, out, want_lse)
+    return _attention(q, k, v, heads, C // heads, scale, kv_segments, out, want_lse)
+
+
 def attention_d64(q, k, v, heads, scale, kv_segments=1, out=None, want_lse=False):
     """q: [B,Lq,>=heads*64] view, k/v: [B,Lk,...] views (fp16, last dim contiguous) -> [B,Lq,heads*64].
     `want_lse`: also return the log2-domain log-sum-exp of the scaled scores, fp32 [B, heads, Lq]
     (P_ij = exp2(scale * log2(e) * S_ij - lse_i)) for the backward pass."""
+    return _attention(q, k, v, heads, 64, scale, kv_segments, out, want_lse)
+
+
+@_timed("attention")
+def _attention(q, k, v, heads, D, scale, kv_segments, out, want_lse):
     _need_cuda(q, k, v)
     assert q.dtype == F16 and k.dtype == F16 and v.dtype == F16
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
     B, Lq = q.shape[0], q.shape[1]
     Lk = k.shape[1]
     if out is None:
-        out = torch.empty((B, Lq, heads * 64), dtype=F16, device=q.device)
+        out = torch.empty((B, Lq, heads * D), dtype=F16, device=q.device)
     kb = k.stride(0) if k.shape[0] > 1 else k.stride(1) * Lk
     vb = v.stride(0) if v.shape[0] > 1 else v.stride(1) * Lk
     qb = q.stride(0) if B > 1 else q.stride(1) * Lq
     lse = torch.empty((B, heads, Lq), dtype=F32, device=q.device) if want_lse else None
-    rc = _lib.load().b200_attention_d64(_p(q), qb, q.stride(1), _p(k), kb, k.stride(1), _p(v), vb, v.stride(1),
-                                        _p(out), out.stride(0) if B > 1 else out.stride(1) * Lq, out.stride(1),
-                                        B, heads, Lq, Lk, kv_segments, float(scale), _p(lse), _stream())
-    _lib.check(rc, "b200_attention_d64")
-    STATS.add("attn", 4 * B * heads * Lq * Lk * kv_segments * 64)
+    rc = _lib.load().b200_attention(_p(q), qb, q.stride(1), _p(k), kb, k.stride(1), _p(v), vb, v.stride(1),
+                                    _p(out), out.stride(0) if B > 1 else out.stride(1) * Lq, out.stride(1),
+                                    B, heads, D, Lq, Lk, kv_segments, float(scale), _p(lse), _stream())
+    _lib.check(rc, "b200_attention")
+    STATS.add("attn", 4 * B * heads * Lq * Lk * kv_segments * D)
     return (out, lse) if want_lse else out
 
 
@@ -365,15 +387,27 @@ def attention_d512(q, k, v, scale, out=None):
     return out
 
 
-@_timed("bwd_misc")
 def rowdot_heads(a, c, heads):
     """delta[b, h, t] = sum_d a[b, t, h*64+d] * c[b, t, h*64+d]; a, c fp16 [B, L, >=heads*64] views -> fp32 [B, heads, L]."""
+    return _rowdot_heads(a, c, heads, 64)
+
+
+def rowdot_heads_d(a, c, heads, head_dim):
+    """delta[b, h, t] = sum_d a[b, t, h*D+d] * c[b, t, h*D+d] with D = head_dim in HEAD_DIMS; a, c fp16
+    [B, L, >=heads*D] views -> fp32 [B, heads, L].  Width 64 is `rowdot_heads`."""
+    if head_dim == 64:
+        return rowdot_heads(a, c, heads)
+    return _rowdot_heads(a, c, heads, head_dim)
+
+
+@_timed("bwd_misc")
+def _rowdot_heads(a, c, heads, head_dim):
     _need_cuda(a, c)
     assert a.dtype == F16 and c.dtype == F16 and a.stride(-1) == 1 and c.stride(-1) == 1 and a.shape[:2] == c.shape[:2]
     B, L = a.shape[0], a.shape[1]
     out = torch.empty((B, heads, L), dtype=F32, device=a.device)
-    _ck(_lib.load().b200_rowdot_heads(_p(a), a.stride(0), a.stride(1), _p(c), c.stride(0), c.stride(1), B, L, heads,
-                                      _p(out), _stream()), "b200_rowdot_heads")
+    _ck(_lib.load().b200_rowdot_heads_d(_p(a), a.stride(0), a.stride(1), _p(c), c.stride(0), c.stride(1), B, L, heads,
+                                        int(head_dim), _p(out), _stream()), "b200_rowdot_heads_d")
     return out
 
 

@@ -39,28 +39,28 @@ class TimestepEmbedding(nn.Module):
 class _DownBlock(nn.Module):
     """CrossAttnDownBlock2D (unet_2d_blocks.py:1027-1185) / DownBlock2D (:1188-1273)."""
 
-    def __init__(self, cin, cout, temb, n, heads, cross_dim, has_attn, add_down, groups, eps, joint):
+    def __init__(self, cin, cout, temb, n, heads, cross_dim, has_attn, add_down, groups, eps, joint, linear_proj):
         super().__init__()
         self.resnets = nn.ModuleList(
             [ResnetBlock2D(cin if i == 0 else cout, cout, temb, groups, eps) for i in range(n)])
         self.attentions = nn.ModuleList(
-            [Transformer2DModel(cout, heads, cross_dim, groups, joint) for _ in range(n)]) if has_attn else None
+            [Transformer2DModel(cout, heads, cross_dim, groups, joint, linear_proj) for _ in range(n)]) if has_attn else None
         self.downsamplers = nn.ModuleList([Downsample2D(cout, 1)]) if add_down else None
 
 
 class _MidBlock(nn.Module):
     """UNetMidBlock2DCrossAttn (unet_2d_blocks.py:634-777)."""
 
-    def __init__(self, ch, temb, heads, cross_dim, groups, eps, joint):
+    def __init__(self, ch, temb, heads, cross_dim, groups, eps, joint, linear_proj):
         super().__init__()
         self.resnets = nn.ModuleList([ResnetBlock2D(ch, ch, temb, groups, eps) for _ in range(2)])
-        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, cross_dim, groups, joint)])
+        self.attentions = nn.ModuleList([Transformer2DModel(ch, heads, cross_dim, groups, joint, linear_proj)])
 
 
 class _UpBlock(nn.Module):
     """CrossAttnUpBlock2D (unet_2d_blocks.py:2201-2371) / UpBlock2D (:2374-2481)."""
 
-    def __init__(self, cin, cout, cprev, temb, n, heads, cross_dim, has_attn, add_up, groups, eps, joint):
+    def __init__(self, cin, cout, cprev, temb, n, heads, cross_dim, has_attn, add_up, groups, eps, joint, linear_proj):
         super().__init__()
         rs = []
         for i in range(n):
@@ -69,7 +69,7 @@ class _UpBlock(nn.Module):
             rs.append(ResnetBlock2D(rin + skip, cout, temb, groups, eps))
         self.resnets = nn.ModuleList(rs)
         self.attentions = nn.ModuleList(
-            [Transformer2DModel(cout, heads, cross_dim, groups, joint) for _ in range(n)]) if has_attn else None
+            [Transformer2DModel(cout, heads, cross_dim, groups, joint, linear_proj) for _ in range(n)]) if has_attn else None
         self.upsamplers = nn.ModuleList([Upsample2D(cout)]) if add_up else None
 
 
@@ -98,14 +98,17 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
         for k in ("block_out_channels", "down_block_types", "up_block_types", "attention_head_dim"):
             if isinstance(cfg[k], list):
                 cfg[k] = tuple(cfg[k])
-        if not cfg["flip_sin_to_cos"] or cfg["freq_shift"] != 0 or not cfg["use_linear_projection"]:
-            raise NotImplementedError("engine supports the SD-2 embedding / linear-projection config only")
+        if not cfg["flip_sin_to_cos"] or cfg["freq_shift"] != 0:
+            raise NotImplementedError("engine supports the SD embedding config (flip_sin_to_cos, freq_shift 0) only")
         self.config = cfg
         self.stream_dtype = stream_dtype
         boc = tuple(cfg["block_out_channels"])
-        heads = tuple(cfg["attention_head_dim"])       # number of heads (unet_2d_condition.py:244-250)
+        # number of heads per block (unet_2d_condition.py:244-250); SD-1 configs store one scalar for all blocks
+        heads = cfg["attention_head_dim"]
+        heads = (heads,) * len(boc) if isinstance(heads, int) else tuple(heads)
         temb = boc[0] * 4
         g, eps, cd, J = cfg["norm_num_groups"], cfg["norm_eps"], cfg["cross_attention_dim"], cfg["joint_attention"]
+        lp = bool(cfg["use_linear_projection"])         # False: 1x1-conv proj_in / proj_out (SD-1, GeoWizard)
         self.conv_in = nn.Conv2d(cfg["in_channels"], boc[0], 3, padding=1)
         self.time_embedding = TimestepEmbedding(boc[0], temb)
         self.class_embedding = (TimestepEmbedding(cfg["projection_class_embeddings_input_dim"], temb)
@@ -115,16 +118,16 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
         for i, t in enumerate(cfg["down_block_types"]):
             cin, ch = ch, boc[i]
             downs.append(_DownBlock(cin, ch, temb, n, heads[i], cd, t == "CrossAttnDownBlock2D",
-                                    i != len(boc) - 1, g, eps, J))
+                                    i != len(boc) - 1, g, eps, J, lp))
         self.down_blocks = nn.ModuleList(downs)
-        self.mid_block = _MidBlock(boc[-1], temb, heads[-1], cd, g, eps, J)
+        self.mid_block = _MidBlock(boc[-1], temb, heads[-1], cd, g, eps, J, lp)
         rev, rheads = list(reversed(boc)), list(reversed(heads))
         ups, cout = [], rev[0]
         for i, t in enumerate(cfg["up_block_types"]):
             cprev, cout = cout, rev[i]
             cin = rev[min(i + 1, len(boc) - 1)]
             ups.append(_UpBlock(cin, cout, cprev, temb, n + 1, rheads[i], cd, t == "CrossAttnUpBlock2D",
-                                i != len(boc) - 1, g, eps, J))
+                                i != len(boc) - 1, g, eps, J, lp))
         self.up_blocks = nn.ModuleList(ups)
         self.conv_norm_out = nn.GroupNorm(g, boc[0], eps=eps)
         self.conv_out = nn.Conv2d(boc[0], cfg["out_channels"], 3, padding=1)

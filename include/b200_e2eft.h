@@ -122,21 +122,30 @@ int b200_group_norm_apply_cs(const void* x1, int C1, const double* cs1, const vo
 int b200_layer_norm(const void* x, int in_f32, long long rows, int C, const float* gamma,
                     const float* beta, float eps, void* y, void* stream);
 
-/* Flash attention, head_dim 64, fp16 Q/K/V read in place from (possibly fused) projection
- * buffers: element (b, l, h, d) of Q is q[b*q_bs + l*q_ls + h*64 + d] (same for K, V).
+/* Flash attention over heads of width head_dim in {40, 64, 80, 160} (ABI 14; any other width returns a negative
+ * code before launch), fp16 Q/K/V read in place from (possibly fused) projection buffers: element (b, l, h, d) of Q
+ * is q[b*q_bs + l*q_ls + h*head_dim + d] (same for K, V).  head_dim 40 / 80 / 160 are the SD-1.x UNet's 320 / 640 /
+ * 1280 channels over 8 heads (GeoWizard); 64 is SD-2's.
  * `kv_segments` = 2 implements GeoWizard's joint self-attention: batch element b attends to the
  * keys/values of b%(B/2) and b%(B/2)+B/2 concatenated (attention.py:482-491).
- * out[b][l][h*64+d] fp16 with row stride o_ls.   softmax(QK^T*scale)V, fp32 softmax.
+ * out[b][l][h*head_dim+d] fp16 with row stride o_ls.   softmax(QK^T*scale)V, fp32 softmax.
+ * Strides are multiples of 8 elements, pointers 16-byte aligned, 1 <= B, heads <= 65535.
  * Replaces xformers.ops.memory_efficient_attention (attention.py:497) / attn1, attn2
  * (attention.py:338-343,375-380). */
+int b200_attention(const void* q, long long q_bs, long long q_ls,
+                   const void* k, long long k_bs, long long k_ls,
+                   const void* v, long long v_bs, long long v_ls,
+                   void* out, long long o_bs, long long o_ls,
+                   int B, int heads, int head_dim, int Lq, int Lk, int kv_segments, float scale,
+                   float* lse /* optional [B][heads][Lq] fp32: log2-domain log-sum-exp of the scaled scores, so that
+                                 P_ij = exp2(scale * log2(e) * S_ij - lse_i) — the backward pass recomputes P from it */,
+                   void* stream);
+/* b200_attention with head_dim = 64. */
 int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
                        const void* k, long long k_bs, long long k_ls,
                        const void* v, long long v_bs, long long v_ls,
                        void* out, long long o_bs, long long o_ls,
-                       int B, int heads, int Lq, int Lk, int kv_segments, float scale,
-                       float* lse /* optional [B][heads][Lq] fp32: log2-domain log-sum-exp of the scaled scores, so that
-                                     P_ij = exp2(scale * log2(e) * S_ij - lse_i) — the backward pass recomputes P from it */,
-                       void* stream);
+                       int B, int heads, int Lq, int Lk, int kv_segments, float scale, float* lse, void* stream);
 
 /* Flash attention, one head of width 512 (the VAE mid-block), fp16 Q/K/V read in place from a
  * (possibly fused) projection buffer: element (b, l, d) of Q is q[b*q_bs + l*q_ls + d] (same for K, V).
@@ -284,8 +293,11 @@ int b200_adamw_step_state_groups(float* param, const float* grad, float* exp_avg
 int b200_gather_planar(const void* x, int in_f32, long long ldx, int NB, int H, int W, int C, int Ho, int Wo, int stride, int up,
                        int oy, int ox, void* out, long long ldo, void* stream);
 int b200_col_sum(const void* x, int in_f32, long long rows, int C, long long ld, float* out, void* stream);
-/* delta[b][h][t] = sum_d a[b,t,h*64+d] * c[b,t,h*64+d] (fp16 in, fp32 out): the row term of the softmax backward,
- * dS = scale * P o (dP - delta), with a = dO and c = O (attention backward, attention.py:497). */
+/* delta[b][h][t] = sum_d a[b,t,h*D+d] * c[b,t,h*D+d] (fp16 in, fp32 out), D = head_dim in {40, 64, 80, 160} (ABI 14):
+ * the row term of the softmax backward, dS = scale * P o (dP - delta), with a = dO and c = O (attention backward,
+ * attention.py:497).  b200_rowdot_heads is the head_dim = 64 call. */
+int b200_rowdot_heads_d(const void* a, long long a_bs, long long a_ls, const void* c, long long c_bs, long long c_ls,
+                        int B, int L, int heads, int head_dim, float* out, void* stream);
 int b200_rowdot_heads(const void* a, long long a_bs, long long a_ls, const void* c, long long c_bs, long long c_ls,
                       int B, int L, int heads, float* out, void* stream);
 int b200_group_norm_mean_rstd(const double* sums, const double* cs1, int C1, const double* cs2, int C2, int NB, int HW,
