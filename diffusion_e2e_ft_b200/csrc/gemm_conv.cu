@@ -215,7 +215,7 @@ extern "C" int b200_debug_last_launch(int* out, int n) {
   memcpy(out, b200::g_last_launch, k * sizeof(int));
   return kLastLaunchFields;
 }
-extern "C" int b200_abi_version(void) { return 14; }
+extern "C" int b200_abi_version(void) { return 15; }
 // Tile width used by the GEGLU epilogue for a packed width N (= 2 x output width); weights must be
 // packed per tile as [value half | gate half] with this width.
 extern "C" int b200_geglu_block_n(int N) {

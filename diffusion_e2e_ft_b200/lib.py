@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 14       # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 15       # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -105,6 +105,13 @@ _SIGS = {
     "b200_eval_normal_error": (c_int, [_P, POINTER(c_longlong), _P, POINTER(c_longlong), _P, c_int, c_int, c_int, _P,
                                        _P, _LL, _P, _P, _P, _P, _P]),
     "b200_eval_kth_smallest": (c_int, [_P, _P, _LL, _LL, _P, _P, _P]),
+    "b200_data_hypersim_source": (c_int, [_P, _P, _P, c_int, c_int, c_int, POINTER(c_double), _P, _P, _P]),
+    "b200_data_resize_u8": (c_int, [_P, c_int, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P, _P, c_int, _P, _P,
+                                    _P, _P]),
+    "b200_data_depth_gather": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, _P, _P, _P]),
+    "b200_data_depth_range": (c_int, [_P, c_int, _LL, c_float, c_float, _P, _P, _P]),
+    "b200_data_finalise": (c_int, [_P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, c_int, c_float, c_float,
+                                   _P, _P, _P, _P, _P, _P, _P, _P]),
 }
 EXPORTS = tuple(_SIGS)
 

@@ -471,6 +471,42 @@ int b200_eval_normal_error(const float* pred, const long long* pred_strides, con
 int b200_eval_kth_smallest(const float* x, const unsigned long long* n, long long n_max, long long k,
                            unsigned long long* ws, float* out, void* stream);
 
+/* Training-batch preparation (ABI 15): the per-sample transforms of training/dataloaders/load.py on decoded images,
+ * bitwise as the reference computes them.  Images are uint8 [B][H][W][3] (HWC), depths uint16 [B][H][W]; flip
+ * (nullable = no sample flipped) is one byte per sample, nonzero = horizontally flipped.  Nothing syncs the host.
+ *
+ * b200_data_hypersim_source: depth_m = float32(mm / 1000.0); the normals re-oriented towards the camera as
+ *   Hypersim.align_normals does in fp64 (inv_k: the 3x3 inverse intrinsics, row-major, on the host) and re-quantised
+ *   to uint8 by truncation; then 255 - x on flipped samples.  normal_out [B][H][W][3] (the flip itself is applied by
+ *   the readers below).
+ * b200_data_resize_u8: Pillow's BILINEAR resize of uint8 [B][H][W][C] to [B][OH][OW][C]: the horizontal pass into
+ *   tmp [B][H][OW][C], then the vertical pass.  Output o of an axis reads taps min[o] + j, j < ks, with 22-bit
+ *   weights k[o * ks + j] (host-built tables on the device); flipped samples read mirrored source columns.
+ * b200_data_depth_gather: dst [B][OH][OW] fp32 = src[b][rows[i]][cols[j]] (column W - 1 - cols[j] when flipped), from
+ *   src_m (fp32 metres) or src_cm (uint16 centimetres, float32(cm) / 100.0) -- exactly one non-NULL.
+ * b200_data_depth_range: per image, over the pixels near < d < far of depth [B][HW]: torch.quantile at 0.02 and 0.98
+ *   (fp32 rank q * (n - 1), torch's fused CPU lerp) into range [B][2]; flag[B] = 0 (no valid pixel), 1 (min == max)
+ *   or 2.
+ * b200_data_finalise: per output pixel of load.py:248-281: rgb / normal read at (top + i, left + j) of [B][H][W][3]
+ *   (mirrored, and 255 - x on the normal, when flipped); depth [B][OH][OW] from b200_data_depth_gather.  Writes
+ *   rgb_out [B][3][OH][OW] = x / 255 * 2 - 1, the valid mask [B][OH][OW] (bytes), metric [B][OH][OW] (clamped, invalid
+ *   pixels at max), depth_out [B][3][OH][OW] normalised to [-1, 1], normal_out [B][3][OH][OW] (F.normalize, zero where
+ *   invalid); flag 0 / 1 give zero depth and metric, flag 1 also an empty mask. */
+int b200_data_hypersim_source(const unsigned short* depth_mm, const unsigned char* normal, const unsigned char* flip,
+                              int B, int H, int W, const double* inv_k, float* depth_m, unsigned char* normal_out,
+                              void* stream);
+int b200_data_resize_u8(const unsigned char* src, int B, int H, int W, int C, int OH, int OW, const int* xmin,
+                        const int* xk, int xks, const int* ymin, const int* yk, int yks, const unsigned char* flip,
+                        unsigned char* tmp, unsigned char* dst, void* stream);
+int b200_data_depth_gather(const float* src_m, const unsigned short* src_cm, int B, int H, int W, int OH, int OW,
+                           const int* rows, const int* cols, const unsigned char* flip, float* dst, void* stream);
+int b200_data_depth_range(const float* depth, int B, long long HW, float near_plane, float far_plane, float* range,
+                          int* flag, void* stream);
+int b200_data_finalise(const unsigned char* rgb, const unsigned char* normal, int B, int H, int W, int top, int left,
+                       const unsigned char* flip, const float* depth, int OH, int OW, float near_plane,
+                       float far_plane, const float* range, const int* flag, float* rgb_out, float* depth_out,
+                       float* metric_out, float* normal_out, unsigned char* mask_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
