@@ -5,8 +5,10 @@
 //   b200_data_depth_gather     Pillow's NEAREST resize of the depth, or the KITTI benchmark crop; the flip folded in
 //   b200_data_depth_range      torch.quantile(valid, 0.02 / 0.98) per image (segmented radix select)
 //   b200_data_finalise         load.py:248-281 / :343-376 per output pixel
-// All HBM-bound.  Per-pixel arithmetic the reference does in fp32 / fp64 is written with explicitly rounded intrinsics
-// so nvcc cannot contract it into FMAs: the outputs are bitwise those of the reference.  Nothing syncs the host.
+//   b200_data_vkitti_normals   the D2NT v3 normals of depth-to-normal-translator/python/gen_vkitti_normals.py
+// All HBM-bound but the last, which is most likely fp64-bound.  Per-pixel arithmetic the reference does in fp32 / fp64 is written
+// with explicitly rounded intrinsics so nvcc cannot contract it into FMAs: the outputs are bitwise those of the
+// reference.  Nothing syncs the host.
 #include "common.cuh"
 #include "../../include/b200_e2eft.h"
 
@@ -268,9 +270,204 @@ __global__ void data_finalise_kernel(const unsigned char* __restrict__ rgb, cons
   }
 }
 
+// ------------------------------------------------------------------------------------ Virtual KITTI 2 normals
+// D2NT "v3" of depth-to-normal-translator/python/gen_vkitti_normals.py:97-136 (DAG-filtered gradients, the
+// depth-to-normal translation, the DLF-alpha MRF refinement) per pixel, in the script's precisions (DESIGN.md §3.11).
+// A CTA owns a kNrmTW x kNrmTH output tile and holds the fp32 depth of the tile plus a 3-pixel halo in shared memory
+// (BORDER_REFLECT_101 applied at load).  Each thread picks its MRF candidate first and then computes the D2NT normal
+// of that one pixel only: the refinement copies a neighbour's normal, so no other normal is needed.
+constexpr int kNrmTW = 32, kNrmTH = 8, kNrmHalo = 3;
+constexpr int kNrmSW = kNrmTW + 2 * kNrmHalo, kNrmSH = kNrmTH + 2 * kNrmHalo;
+constexpr double kLnE32Hi = 0x1.fffffefb245eap-1;     // ln(float32(e)) = kLnE32Hi + kLnE32Lo (double-double)
+constexpr double kLnE32Lo = 0x1.a2d208d1c4e82p-56;
+constexpr double kLn2Hi = 0.6931471805599453, kLn2Lo = 2.3190468138462996e-17;
+
+struct DD { double hi, lo; };
+
+__device__ __forceinline__ DD quick_two_sum(double a, double b) {
+  const double s = __dadd_rn(a, b);
+  return {s, __dsub_rn(b, __dsub_rn(s, a))};
+}
+__device__ __forceinline__ DD two_sum(double a, double b) {
+  const double s = __dadd_rn(a, b), bb = __dsub_rn(s, a);
+  return {s, __dadd_rn(__dsub_rn(a, __dsub_rn(s, bb)), __dsub_rn(b, bb))};
+}
+__device__ __forceinline__ DD dd_add(DD a, DD b) {
+  DD s = two_sum(a.hi, b.hi);
+  const DD t = two_sum(a.lo, b.lo);
+  s = quick_two_sum(s.hi, __dadd_rn(s.lo, t.hi));
+  return quick_two_sum(s.hi, __dadd_rn(s.lo, t.lo));
+}
+__device__ __forceinline__ DD dd_mul(DD a, DD b) {
+  const double p = __dmul_rn(a.hi, b.hi);
+  double e = __fma_rn(a.hi, b.hi, -p);
+  e = __dadd_rn(e, __dadd_rn(__dmul_rn(a.hi, b.lo), __dmul_rn(a.lo, b.hi)));
+  return quick_two_sum(p, e);
+}
+__device__ __forceinline__ DD dd_mul_d(DD a, double b) {
+  const double p = __dmul_rn(a.hi, b);
+  return quick_two_sum(p, __fma_rn(a.lo, b, __fma_rn(a.hi, b, -p)));
+}
+__device__ __forceinline__ DD dd_div_d(DD a, double b) {
+  const double q1 = __ddiv_rn(a.hi, b);
+  const double p = __dmul_rn(q1, b), pe = __fma_rn(q1, b, -p);
+  const double r = __dadd_rn(__dsub_rn(__dsub_rn(a.hi, p), pe), a.lo);
+  return quick_two_sum(q1, __ddiv_rn(r, b));
+}
+
+// exp(t) for a double-double t in about [-745, 0], to ~2^-95 relative: t = k ln2 + r, exp(r) = exp(r / 512)^512 with a
+// degree-12 Taylor polynomial of exp(r / 512).
+__device__ __forceinline__ DD dd_exp(DD t) {
+  const double k = rint(__dmul_rn(t.hi, 1.4426950408889634));
+  const DD r = dd_add(t, dd_mul_d(DD{-kLn2Hi, -kLn2Lo}, k));
+  const DD s{r.hi * 0x1p-9, r.lo * 0x1p-9};
+  DD acc{1.0, 0.0};
+  for (int n = 12; n >= 1; --n) acc = dd_add(DD{1.0, 0.0}, dd_div_d(dd_mul(s, acc), (double)n));
+  for (int i = 0; i < 9; ++i) acc = dd_mul(acc, acc);
+  return {scalbn(acc.hi, (int)k), scalbn(acc.lo, (int)k)};
+}
+
+// float32(e) ** -x correctly rounded to fp32 (x >= 0 finite), returned widened to double.  soft_min's np.power runs
+// in fp32 and is not correctly rounded on every CPU; this is the value its correctly rounded counterpart gives.  The
+// fast path is exp() of the double-double argument -x ln(float32(e)), good to < 2^-51 relative; when that is within
+// 2^-46 of an fp32 rounding boundary the double-double exp decides.  Subnormal results are kept.  force_slow takes the
+// double-double path for every x and *slow reports whether it was taken (both only for b200_debug_pow_e32_neg).
+__device__ __forceinline__ double pow_e32_neg(float x, bool force_slow = false, bool* slow = nullptr) {
+  const double nx = -(double)x;
+  const double th = __dmul_rn(nx, kLnE32Hi);
+  const double tl = __fma_rn(nx, kLnE32Lo, __fma_rn(nx, kLnE32Hi, -th));
+  const double e = exp(th);
+  const double y = __fma_rn(e, tl, e);
+  const float a = __double2float_rn(__dmul_rn(y, 1.0 - 0x1p-46)), b = __double2float_rn(__dmul_rn(y, 1.0 + 0x1p-46));
+  if (a == b && !force_slow) return (double)a;
+  if (slow) *slow = true;
+  const DD v = dd_exp(DD{th, tl});
+  const float lo = __double2float_rd(v.hi), hi = __double2float_ru(v.hi);
+  if (lo == hi) return (double)lo;
+  const double d = __dadd_rn(__dsub_rn(v.hi, __dmul_rn(__dadd_rn((double)lo, (double)hi), 0.5)), v.lo);
+  if (d != 0.0) return (double)(d > 0.0 ? hi : lo);
+  return (double)((__float_as_uint(lo) & 1u) ? hi : lo);
+}
+
+// soft_min's weights of one direction followed by get_DAG_filter's four in-place threshold updates (myApis.py:48-70,
+// :112-120), in fp64; pa / pb are the powers of the laplacian one pixel before / after (0 off the image).
+__device__ __forceinline__ void dag_weights(double pa, double pb, double& wa, double& wb) {
+  const double eps = 1e-8, E = 2.718281828459045;
+  const double den = __dadd_rn(__dadd_rn(eps, pa), pb);
+  wa = __ddiv_rn(__dadd_rn(pa, eps * 0.5), den);
+  wb = __ddiv_rn(__dadd_rn(pb, eps * 0.5), den);
+  if (__ddiv_rn(wa, __dadd_rn(wb, eps)) > E) wa = 1.0;
+  if (__ddiv_rn(wa, __dadd_rn(wb, eps)) > E) wb = 0.0;
+  if (__ddiv_rn(wb, __dadd_rn(wa, eps)) > E) wa = 0.0;
+  if (__ddiv_rn(wb, __dadd_rn(wa, eps)) > E) wb = 1.0;
+}
+
+__global__ void __launch_bounds__(kNrmTW * kNrmTH)
+data_vkitti_normals_kernel(const unsigned short* __restrict__ depth_cm, int H, int W, float fx, float fy, float u0,
+                           float v0, unsigned short* __restrict__ out) {
+  __shared__ float z[kNrmSH][kNrmSW];
+  const int b = blockIdx.z, x0 = blockIdx.x * kNrmTW, y0 = blockIdx.y * kNrmTH;
+  const unsigned short* src = depth_cm + (long long)b * H * W;
+  for (int t = threadIdx.y * kNrmTW + threadIdx.x; t < kNrmSH * kNrmSW; t += kNrmTW * kNrmTH) {
+    int gy = y0 - kNrmHalo + t / kNrmSW, gx = x0 - kNrmHalo + t % kNrmSW;
+    gy = gy < 0 ? -gy : (gy >= H ? 2 * H - 2 - gy : gy);   // BORDER_REFLECT_101; only distance 1 is ever read
+    gx = gx < 0 ? -gx : (gx >= W ? 2 * W - 2 - gx : gx);
+    gy = min(max(gy, 0), H - 1);
+    gx = min(max(gx, 0), W - 1);
+    // cv2.imread -> float32 / 100 (gen_vkitti_normals.py:63) -> ToTensor -> * 100 (:100)
+    z[t / kNrmSW][t % kNrmSW] = __fmul_rn(__fdiv_rn((float)src[(long long)gy * W + gx], 100.0f), 100.0f);
+  }
+  __syncthreads();
+  const int py = y0 + threadIdx.y, px = x0 + threadIdx.x;
+  if (py >= H || px >= W) return;
+  const int ty = threadIdx.y + kNrmHalo, tx = threadIdx.x + kNrmHalo;
+
+  // MRF_optim (DLF-alpha): |cv2.filter2D(depth, lap_ker_alpha)| summed as cv2 does, of [left, right, up, down,
+  // self]; off-image candidates are +inf and argmin keeps the first minimum
+  auto lap_alpha = [&](int cy, int cx) {
+    const float s = __fsub_rn(__fsub_rn(__fadd_rn(__fsub_rn(__fsub_rn(0.0f, z[cy - 1][cx]), z[cy][cx - 1]),
+                                                  __fmul_rn(4.0f, z[cy][cx])), z[cy][cx + 1]), z[cy + 1][cx]);
+    return fabsf(s);
+  };
+  const float inf = __int_as_float(0x7f800000);
+  const float cand[5] = {px > 0 ? lap_alpha(ty, tx - 1) : inf, px < W - 1 ? lap_alpha(ty, tx + 1) : inf,
+                         py > 0 ? lap_alpha(ty - 1, tx) : inf, py < H - 1 ? lap_alpha(ty + 1, tx) : inf,
+                         lap_alpha(ty, tx)};
+  int best = 0;
+  float least = cand[0];
+#pragma unroll
+  for (int k = 1; k < 5; ++k)
+    if (cand[k] < least) {
+      least = cand[k];
+      best = k;
+    }
+  const int qy = ty + (best == 2 ? -1 : best == 3 ? 1 : 0), qx = tx + (best == 0 ? -1 : best == 1 ? 1 : 0);
+  const int gy = py + (qy - ty), gx = px + (qx - tx);
+
+  // get_DAG_filter (1D-DLF) at q: one-sided fp32 gradients, their fp32 laplacians one pixel either side
+  auto grad_l = [&](int cy, int cx) { return __fsub_rn(z[cy][cx], z[cy][cx - 1]); };
+  auto grad_u = [&](int cy, int cx) { return __fsub_rn(z[cy][cx], z[cy - 1][cx]); };
+  auto lap_hor = [&](int cy, int cx) { return fabsf(__fsub_rn(grad_l(cy, cx), grad_l(cy, cx + 1))); };
+  auto lap_ver = [&](int cy, int cx) { return fabsf(__fsub_rn(grad_u(cy, cx), grad_u(cy + 1, cx))); };
+  double l1, l2, l3, l4;
+  dag_weights(gx > 0 ? pow_e32_neg(lap_hor(qy, qx - 1)) : 0.0, gx < W - 1 ? pow_e32_neg(lap_hor(qy, qx + 1)) : 0.0,
+              l1, l2);
+  dag_weights(gy > 0 ? pow_e32_neg(lap_ver(qy - 1, qx)) : 0.0, gy < H - 1 ? pow_e32_neg(lap_ver(qy + 1, qx)) : 0.0,
+              l3, l4);
+  const double Gu = __dadd_rn(__dmul_rn(l1, (double)grad_l(qy, qx)), __dmul_rn(l2, (double)grad_l(qy, qx + 1)));
+  const double Gv = __dadd_rn(__dmul_rn(l3, (double)grad_u(qy, qx)), __dmul_rn(l4, (double)grad_u(qy + 1, qx)));
+
+  // translation (:116-118) and vector_normalization (apis.py:38-41), fp64
+  const double um = __dsub_rn((double)(gx + 1), (double)u0), vm = __dsub_rn((double)(gy + 1), (double)v0);
+  const double n[3] = {__dmul_rn(Gu, (double)fx), __dmul_rn(Gv, (double)fy),
+                       -__dadd_rn(__dadd_rn((double)z[qy][qx], __dmul_rn(vm, Gv)), __dmul_rn(um, Gu))};
+  const double mag = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(n[0], n[0]), __dmul_rn(n[1], n[1])),
+                                          __dmul_rn(n[2], n[2])));
+  const double den = __dadd_rn(mag, 1e-8);
+  // uint16((-n + 1) * 32767.5), truncated, stored in cvtColor(RGB2BGR) order: z, y, x
+  unsigned short* o = out + (((long long)b * H + py) * W + px) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+    o[2 - c] = (unsigned short)__double2uint_rz(__dmul_rn(__dadd_rn(-__ddiv_rn(n[c], den), 1.0), 32767.5));
+}
+
+// out[i] = pow_e32_neg(x[i]); counts in *slow_count (nullable) how many took the double-double path
+__global__ void debug_pow_e32_neg_kernel(const float* __restrict__ x, long long n, int force_slow,
+                                         float* __restrict__ out, unsigned int* __restrict__ slow_count) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    bool slow = false;
+    out[i] = (float)pow_e32_neg(x[i], force_slow != 0, &slow);
+    if (slow && slow_count) atomicAdd(slow_count, 1u);
+  }
+}
+
 }  // namespace b200
 
 using namespace b200;
+
+extern "C" int b200_debug_pow_e32_neg(const float* x, long long n, int force_slow, float* out,
+                                      unsigned int* slow_count, void* stream) {
+  B200_CHECK_ARG(x && out, "b200_debug_pow_e32_neg: null pointer");
+  B200_CHECK_ARG(n >= 1, "b200_debug_pow_e32_neg: n=%lld", n);
+  debug_pow_e32_neg_kernel<<<data_grid(n), kDataThreads, 0, (cudaStream_t)stream>>>(x, n, force_slow, out, slow_count);
+  B200_CHECK_LAUNCH("debug_pow_e32_neg_kernel");
+  return 0;
+}
+
+extern "C" int b200_data_vkitti_normals(const unsigned short* depth_cm, int B, int H, int W, float fx, float fy,
+                                        float u0, float v0, unsigned short* out, void* stream) {
+  B200_CHECK_ARG(depth_cm && out, "b200_data_vkitti_normals: null pointer");
+  B200_CHECK_ARG(B >= 1 && B <= 65535 && H >= 3 && W >= 3 && (long long)H * W < (1LL << 40),
+                 "b200_data_vkitti_normals: bad shape B=%d H=%d W=%d (H, W >= 3)", B, H, W);
+  B200_CHECK_ARG(isfinite(fx) && isfinite(fy) && isfinite(u0) && isfinite(v0),
+                 "b200_data_vkitti_normals: non-finite intrinsics");
+  const dim3 grid((W + kNrmTW - 1) / kNrmTW, (H + kNrmTH - 1) / kNrmTH, B);
+  B200_CHECK_ARG(grid.y <= 65535, "b200_data_vkitti_normals: H=%d too large", H);
+  data_vkitti_normals_kernel<<<grid, dim3(kNrmTW, kNrmTH), 0, (cudaStream_t)stream>>>(depth_cm, H, W, fx, fy, u0, v0,
+                                                                                      out);
+  B200_CHECK_LAUNCH("data_vkitti_normals_kernel");
+  return 0;
+}
 
 extern "C" int b200_data_hypersim_source(const unsigned short* depth_mm, const unsigned char* normal,
                                          const unsigned char* flip, int B, int H, int W, const double* inv_k,

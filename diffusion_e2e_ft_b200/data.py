@@ -5,18 +5,23 @@ transforms on the device (DESIGN.md §3 "Training inputs").
     MixedDataLoader           <- load.py:18-59
     prepare_batch             <- the rest of __getitem__ (load.py:74-98, :106-152, :187-281, :343-376) plus the
                                  `.to(device)` of the training loop, on a collated batch of one dataset
+    vkitti_normals            <- depth-to-normal-translator/python/gen_vkitti_normals.py:97-136 (D2NT v3) on a batch
+    generate_vkitti_normals   <- the whole of gen_vkitti_normals.py: vkitti_DAG_normals/ written from the depths
 
 A training loop keeps its DataLoaders and swaps `from dataloaders.load import *` for this module, then calls
 `batch = prepare_batch(batch)` on every batch.  The returned dict has the keys, shapes and dtypes the reference's
 collated samples have, and the same values bit for bit; the arithmetic runs in libb200_e2eft.so (csrc/data.cu).
 """
+import collections
 import ctypes
+import math
 import os
 import random
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
-from torch.utils.data import Dataset
+from torch.utils.data import DataLoader, Dataset
 
 from . import lib as _lib
 from .ops import _ck, _p, _stream
@@ -28,6 +33,11 @@ HYPERSIM_CSV = os.path.join("data", "hypersim", "processed", "train", "filename_
 VKITTI_SCENES = ("Scene01", "Scene02", "Scene06", "Scene18", "Scene20")
 VKITTI_WEATHER = ("morning", "fog", "rain", "sunset", "overcast")
 VKITTI_CAMERAS = ("Camera_0", "Camera_1")
+# the ten variants gen_vkitti_normals.py:31 writes normals for (the training loader reads five of them)
+VKITTI_NORMAL_VARIANTS = ("15-deg-left", "15-deg-right", "30-deg-left", "30-deg-right", "clone", "morning", "fog",
+                          "rain", "sunset", "overcast")
+# the Virtual KITTI 2 depth camera as gen_vkitti_normals.py:68-71 gives it (vkitti_2.0.3_textgt)
+VKITTI_FX, VKITTI_FY, VKITTI_U0, VKITTI_V0 = 725.0087, 725.0087, 620.5, 187.0
 _PB = 22                                   # Pillow's PRECISION_BITS for 8-bit resampling
 
 
@@ -166,13 +176,13 @@ class VirtualKITTI2(Dataset):
         self.transform = bool(transform)
         self.pairs = self._find_pairs()
 
-    def _find_pairs(self):
+    def _find_pairs(self, variants=VKITTI_WEATHER):
         rgb_root = os.path.join(self.root_dir, "vkitti_2.0.3_rgb")
         depth_root = os.path.join(self.root_dir, "vkitti_2.0.3_depth")
         normal_root = os.path.join(self.root_dir, "vkitti_DAG_normals")
         pairs = []
         for scene in VKITTI_SCENES:
-            for weather in VKITTI_WEATHER:
+            for weather in variants:
                 for camera in VKITTI_CAMERAS:
                     rgb_dir = os.path.join(rgb_root, scene, weather, "frames", "rgb", camera)
                     depth_dir = os.path.join(depth_root, scene, weather, "frames", "depth", camera)
@@ -370,3 +380,115 @@ def _launch(batch, dev, domain, transform, near, far, hypersim_size):
     out["val_mask"] = mask
     out["domain"] = [domain] * B
     return out
+
+
+# ------------------------------------------------------------------------------------ Virtual KITTI 2 normals
+def vkitti_normals(depth_cm, fx=VKITTI_FX, fy=VKITTI_FY, u0=VKITTI_U0, v0=VKITTI_V0):
+    """D2NT "v3" normals of gen_vkitti_normals.py:97-136 (DAG-filtered gradients, depth-to-normal translation, MRF
+    refinement) for a uint16 [B,H,W] CUDA tensor of centimetre depths -> torch.uint16 [B,H,W,3] on the same device:
+    uint16((-n + 1) * 32767.5) in the channel order the script hands cv2.imwrite (z, y, x; the file's RGB is x, y, z).
+    The intrinsics are taken as float32, as the script's torch tensor holds them.  The result is bitwise the script's
+    with its fp32 np.power(e, -lap) correctly rounded (DESIGN.md §3.11).  Runs under torch.cuda.device(depth.device)
+    on its current stream without syncing the host; bad arguments raise ValueError before any launch."""
+    if not isinstance(depth_cm, torch.Tensor) or depth_cm.dtype != torch.uint16 or depth_cm.dim() != 3:
+        raise ValueError("vkitti_normals takes a uint16 [B,H,W] tensor of centimetre depths, got "
+                         f"{depth_cm.dtype if isinstance(depth_cm, torch.Tensor) else type(depth_cm).__name__} "
+                         f"{tuple(depth_cm.shape) if isinstance(depth_cm, torch.Tensor) else ''}")
+    if not depth_cm.is_cuda:
+        raise ValueError(f"vkitti_normals runs on a CUDA device (no CPU fallback), got {depth_cm.device}")
+    B, H, W = depth_cm.shape
+    if not (1 <= B <= 65535 and H >= 3 and W >= 3):
+        raise ValueError(f"vkitti_normals needs 1 <= B <= 65535 and H, W >= 3, got {tuple(depth_cm.shape)}")
+    cam = [float(v) for v in (fx, fy, u0, v0)]
+    with np.errstate(over="ignore"):
+        finite = all(math.isfinite(v) and np.isfinite(np.float32(v)) for v in cam)
+    if not finite:
+        raise ValueError(f"vkitti_normals needs finite intrinsics, got fx, fy, u0, v0 = {cam}")
+    with torch.cuda.device(depth_cm.device):
+        L = _lib.load()
+        depth = depth_cm.contiguous()
+        out = torch.empty((B, H, W, 3), dtype=torch.uint16, device=depth.device)
+        _ck(L.b200_data_vkitti_normals(_p(depth), B, H, W, *cam, _p(out), _stream()), "b200_data_vkitti_normals")
+    return out
+
+
+class _VKITTIDepthFrames(VirtualKITTI2):
+    """The frames gen_vkitti_normals.py walks (its ten variants) as (normal path, uint16 depth [H,W]); decoded with the
+    script's cv2.imread flags (:62)."""
+
+    def __init__(self, root_dir):
+        self.root_dir = root_dir
+        self.pairs = self._find_pairs(VKITTI_NORMAL_VARIANTS)
+
+    def __getitem__(self, idx):
+        import cv2
+        _, depth_path, normal_path = self.pairs[idx]
+        depth = cv2.imread(depth_path, cv2.IMREAD_ANYCOLOR | cv2.IMREAD_ANYDEPTH)
+        if depth is None or depth.dtype != np.uint16 or depth.ndim != 2:
+            raise ValueError(f"{depth_path}: missing, or not a single-channel 16-bit PNG")
+        return normal_path, torch.from_numpy(depth)
+
+
+def _equal_size_batches(frames, batch_size):
+    """Consecutive frames of one size, at most batch_size at a time: (paths, uint16 [B,H,W])."""
+    paths, depths = [], []
+    for path, depth in frames:
+        if depths and (len(depths) == batch_size or depth.shape != depths[0].shape):
+            yield paths, torch.stack(depths)
+            paths, depths = [], []
+        paths.append(path)
+        depths.append(depth)
+    if depths:
+        yield paths, torch.stack(depths)
+
+
+def _normals_on_host(depth, dev):
+    """uint16 depth [B,H,W] on the host -> its normals, computed on `dev`, as a uint16 [B,H,W,3] numpy array in
+    ordinary host memory.  The copies go through pinned staging buffers that are released on return (the caching
+    host allocator hands them to the next batch), so queued PNG writes never hold page-locked memory."""
+    out = vkitti_normals(depth.pin_memory().to(dev, non_blocking=True))
+    host = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
+    host.copy_(out, non_blocking=True)
+    torch.cuda.current_stream().synchronize()
+    return host.numpy().copy()
+
+
+def _write_png(path, normals):
+    import cv2
+    os.makedirs(os.path.dirname(path), exist_ok=True)
+    if not cv2.imwrite(path, normals):
+        raise OSError(f"cv2.imwrite could not write {path}")
+
+
+def generate_vkitti_normals(root_dir, batch_size=8, num_workers=4, device=None):
+    """What `python gen_vkitti_normals.py` does, on the device: for every frame of the script's walk over root_dir
+    (5 scenes x 10 variants x 2 cameras), the D2NT v3 normals of vkitti_2.0.3_depth/.../depth_*.png written as a
+    16-bit PNG to vkitti_DAG_normals/.../normal_*.png, the path VirtualKITTI2 reads.  DataLoader workers decode, runs of
+    equal-size frames go through vkitti_normals batch_size at a time, and a pool of num_workers threads encodes and
+    writes.  At most 2 * max(batch_size, num_workers) computed frames wait for their write at any time: the loop
+    blocks on the oldest write beyond that, so host memory stays bounded however much slower encoding is than
+    decoding.  Returns the number of frames written.  A missing or non-16-bit depth file raises ValueError naming it."""
+    if batch_size < 1 or num_workers < 0:
+        raise ValueError(f"need batch_size >= 1 and num_workers >= 0, got {batch_size}, {num_workers}")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device()) \
+        if torch.cuda.is_available() else None
+    if dev is None or dev.type != "cuda":
+        raise ValueError(f"generate_vkitti_normals runs on a CUDA device (no CPU fallback), got {dev}")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    frames = DataLoader(_VKITTIDepthFrames(root_dir), batch_size=None, shuffle=False, num_workers=num_workers)
+    max_pending = 2 * max(batch_size, num_workers)
+    written = 0
+    with torch.cuda.device(dev), ThreadPoolExecutor(max(1, num_workers)) as pool:
+        pending = collections.deque()
+        for paths, depth in _equal_size_batches(frames, batch_size):
+            normals = _normals_on_host(depth, dev)
+            for p, n in zip(paths, normals):
+                while len(pending) >= max_pending:
+                    pending.popleft().result()
+                    written += 1
+                pending.append(pool.submit(_write_png, p, n))
+        while pending:
+            pending.popleft().result()
+            written += 1
+    return written

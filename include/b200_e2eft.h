@@ -507,6 +507,20 @@ int b200_data_finalise(const unsigned char* rgb, const unsigned char* normal, in
                        float far_plane, const float* range, const int* flag, float* rgb_out, float* depth_out,
                        float* metric_out, float* normal_out, unsigned char* mask_out, void* stream);
 
+/* Virtual KITTI 2 training normals (ABI 16): D2NT "v3" of depth-to-normal-translator/python/gen_vkitti_normals.py
+ * (DAG-filtered depth gradients, the depth-to-normal translation, the DLF-alpha MRF refinement) on uint16
+ * centimetre depth [B][H][W], H, W >= 3, with intrinsics fx, fy, u0, v0 (float32, as the script's torch tensor holds
+ * them).  out [B][H][W][3] uint16 = (-n + 1) * 32767.5 truncated, in the array order cv2.imwrite takes after the
+ * script's cvtColor(RGB2BGR): z, y, x.  Bitwise the script's output with its fp32 np.power(e, -lap) replaced by the
+ * correctly rounded fp32 value (DESIGN.md §3.11).  Nothing syncs the host. */
+int b200_data_vkitti_normals(const unsigned short* depth_cm, int B, int H, int W, float fx, float fy, float u0,
+                             float v0, unsigned short* out, void* stream);
+/* The kernel's float32(e) ** -x (x >= 0, fp32 [n]) on its own, for testing the correct rounding: out[i] as
+ * b200_data_vkitti_normals computes it; force_slow != 0 takes the double-double path for every element; slow_count
+ * (device, nullable, not reset) is incremented once per element that took the double-double path. */
+int b200_debug_pow_e32_neg(const float* x, long long n, int force_slow, float* out, unsigned int* slow_count,
+                           void* stream);
+
 #ifdef __cplusplus
 }
 #endif
