@@ -315,7 +315,7 @@ __device__ __forceinline__ DD dd_div_d(DD a, double b) {
   return quick_two_sum(q1, __ddiv_rn(r, b));
 }
 
-// exp(t) for a double-double t in about [-745, 0], to ~2^-95 relative: t = k ln2 + r, exp(r) = exp(r / 512)^512 with a
+// exp(t) for a double-double t in about [-745, 709], to ~2^-95 relative: t = k ln2 + r, exp(r) = exp(r / 512)^512 with a
 // degree-12 Taylor polynomial of exp(r / 512).
 __device__ __forceinline__ DD dd_exp(DD t) {
   const double k = rint(__dmul_rn(t.hi, 1.4426950408889634));
@@ -441,6 +441,276 @@ __global__ void debug_pow_e32_neg_kernel(const float* __restrict__ x, long long 
   }
 }
 
+// ------------------------------------------------------------------------------------ Hypersim preprocessing
+// Marigold's preprocess_hypersim.py / hypersim_util.py per frame (DESIGN.md §3.12), in the script's precisions:
+//   brightness = (0.3 r + 0.59 g) + 0.11 b in fp64 over the valid pixels (entity id != -1);
+//   p90 = np.percentile(brightness_valid, 90) (method 'linear'): the two order statistics by an exact radix select
+//         on fp64 keys (8 passes of 8 bits over a per-pixel key buffer), then NumPy's virtual index, gamma and _lerp;
+//   scale = 1 (no valid pixel), 0 (p90 < 1e-4), else pow(0.8, 2.2) / p90 (a NaN p90 gives a NaN scale);
+//   rgb   = uint8(clip(pow(max(scale x, 0), 1 / 2.2), 0, 1) * 255) with the power correctly rounded, stored B, G, R;
+//   depth = uint16(distance / ||(x, y, f)||_fp32 * f * 1000), 0 where invalid.
+// NumPy's float64 -> uint8 / uint16 casts truncate through int32 on x86 and keep the low bits: NaN and anything
+// outside the int32 range give 0, -3.7 gives 65533 (trunc_wrap).
+constexpr int kHsPasses = 8;                           // 8-bit digits of a 64-bit key
+constexpr int kHsHistThreads = 1024, kHsHistCtas = 64;  // per frame
+constexpr unsigned long long kHsNoKey = ~0ull;         // invalid or NaN brightness: never a key of a non-NaN double
+constexpr double kHsGamma = 1.0 / 2.2;                 // the script's gamma, 0.45454545454545453
+
+__device__ __forceinline__ unsigned long long hs_key(double v) {   // orders as the values (-0 before +0)
+  const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+  return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double hs_value(unsigned long long k) {
+  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+__device__ __forceinline__ unsigned int trunc_wrap(double v) {
+  return (v > -2147483649.0 && v < 2147483648.0) ? (unsigned int)(int)v : 0u;
+}
+template <typename T> __device__ __forceinline__ double hs_load(const T* p, long long i);
+template <> __device__ __forceinline__ double hs_load<float>(const float* p, long long i) { return (double)p[i]; }
+template <> __device__ __forceinline__ double hs_load<__half>(const __half* p, long long i) {
+  return (double)__half2float(p[i]);
+}
+
+// The uint8 level of a tone-mapped value p = pow(m, gamma): uint8(clip(p, 0, 1) * 255), NaN -> 0.
+__device__ __forceinline__ unsigned char hs_level(double p) {
+  if (isnan(p)) return 0;
+  return (unsigned char)trunc_wrap(__dmul_rn(fmin(fmax(p, 0.0), 1.0), 255.0));
+}
+
+// pow(m, gamma) for m > 0 finite in double-double: log(m) = e ln2 + log(f), m = f 2^e, f in [1, 2), with log(f) from
+// one Newton step y0 + (f exp(-y0) - 1) on the fp64 log; then dd_exp of gamma log(m).  Good to ~2^-94 relative.
+__device__ __forceinline__ double hs_pow_gamma_dd(double m) {
+  int e;
+  double f = frexp(m, &e);                             // [0.5, 1)
+  f = __dmul_rn(f, 2.0);
+  e -= 1;
+  const double y0 = log(f);
+  const DD ef = dd_mul_d(dd_exp(DD{-y0, 0.0}), f);
+  const DD lf = dd_add(DD{y0, 0.0}, dd_add(ef, DD{-1.0, 0.0}));
+  const DD lm = dd_add(dd_mul_d(DD{kLn2Hi, kLn2Lo}, (double)e), lf);
+  const DD p = dd_exp(dd_mul_d(lm, kHsGamma));
+  return __dadd_rn(p.hi, p.lo);
+}
+
+// The uint8 level of pow(m, gamma) with the power correctly rounded, for m = np.maximum(scale x, 0) (NaN kept).
+// The fast fp64 pow is within a few ulp; when the level differs anywhere in +-2^-48 (relative) of it, the
+// double-double power decides.  *p_out gets the power used; force_slow / *slow are for b200_debug_hypersim_pow.
+__device__ __forceinline__ unsigned char hs_tone(double m, bool force_slow = false, bool* slow = nullptr,
+                                                 double* p_out = nullptr) {
+  double p;
+  if (isnan(m) || m == 0.0 || isinf(m)) {
+    p = isnan(m) ? m : (m == 0.0 ? 0.0 : m);
+  } else {
+    p = pow(m, kHsGamma);
+    const unsigned char lo = hs_level(__dmul_rn(p, 1.0 - 0x1p-48)), hi = hs_level(__dmul_rn(p, 1.0 + 0x1p-48));
+    if (lo != hi || force_slow) {
+      if (slow) *slow = true;
+      p = hs_pow_gamma_dd(m);
+    }
+  }
+  if (p_out) *p_out = p;
+  return hs_level(p);
+}
+
+// Pass 0: one fp64 brightness key per pixel (kHsNoKey where invalid or NaN), the per-frame counts of valid and of
+// NaN-valued valid pixels, and the entity_id == 0 flag the script asserts on.
+template <typename TR>
+__global__ void hs_keys_kernel(const TR* __restrict__ rgb, const int* __restrict__ eid, long long HW,
+                               unsigned long long* __restrict__ keys, unsigned long long* __restrict__ counts,
+                               int* __restrict__ err) {
+  const int b = blockIdx.y;
+  unsigned long long n_valid = 0, n_nan = 0;
+  bool zero = false;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
+    const long long g = (long long)b * HW + i;
+    const int e = eid[g];
+    zero |= e == 0;
+    unsigned long long k = kHsNoKey;
+    if (e != -1) {
+      const double br = __dadd_rn(__dadd_rn(__dmul_rn(0.3, hs_load(rgb, 3 * g)), __dmul_rn(0.59, hs_load(rgb, 3 * g + 1))),
+                                  __dmul_rn(0.11, hs_load(rgb, 3 * g + 2)));
+      ++n_valid;
+      if (isnan(br)) ++n_nan;
+      else k = hs_key(br);
+    }
+    keys[g] = k;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    n_valid += __shfl_xor_sync(0xffffffffu, n_valid, o);
+    n_nan += __shfl_xor_sync(0xffffffffu, n_nan, o);
+  }
+  if (__any_sync(0xffffffffu, zero) && (threadIdx.x & 31) == 0) atomicOr(err + b, 1);
+  if ((threadIdx.x & 31) == 0 && n_valid) {
+    atomicAdd(counts + 2 * b, n_valid);
+    if (n_nan) atomicAdd(counts + 2 * b + 1, n_nan);
+  }
+}
+
+// One radix pass: per frame and wanted rank (0: floor of the virtual index, 1: the next), the histogram of digit
+// `pass` over the keys that share the digits chosen so far.  Warp-aggregated shared-memory counts, then one global
+// atomic per non-empty bin per CTA.  Frames with no valid pixel or a NaN skip the select.
+__global__ void __launch_bounds__(kHsHistThreads)
+hs_hist_kernel(const unsigned long long* __restrict__ keys, long long HW, int pass,
+               const unsigned long long* __restrict__ counts, const unsigned long long* __restrict__ sel,
+               unsigned int* __restrict__ hist) {
+  __shared__ unsigned int h[2 * 256];
+  const int b = blockIdx.y;
+  if (counts[2 * b] == 0 || counts[2 * b + 1] != 0) return;
+  for (int t = threadIdx.x; t < 512; t += blockDim.x) h[t] = 0u;
+  __syncthreads();
+  const int shift = 56 - 8 * pass, hi_shift = shift + 8;
+  const unsigned long long pre[2] = {sel[4 * b], sel[4 * b + 1]};
+  const unsigned long long* k = keys + (long long)b * HW;
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long end = (HW + 31) / 32 * 32;           // whole warps iterate together for __match_any_sync
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < end; i += stride) {
+    const unsigned long long key = i < HW ? k[i] : kHsNoKey;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const bool in = key != kHsNoKey && (pass == 0 || ((key ^ pre[r]) >> hi_shift) == 0ull);
+      const unsigned int bin = in ? (unsigned int)(r * 256 + ((key >> shift) & 255ull)) : 512u;
+      const unsigned int peers = __match_any_sync(0xffffffffu, bin);
+      if (in && (threadIdx.x & 31) == (unsigned)(__ffs(peers) - 1)) atomicAdd(&h[bin], (unsigned)__popc(peers));
+    }
+  }
+  __syncthreads();
+  unsigned int* g = hist + ((long long)pass * gridDim.y + b) * 512;
+  for (int t = threadIdx.x; t < 512; t += blockDim.x)
+    if (h[t]) atomicAdd(g + t, h[t]);
+}
+
+// After pass `pass`: each frame's two wanted ranks choose their digit.  After the last pass the order statistics
+// are known and thread 0 writes stats[b] = (p90, scale): p90 by NumPy's _quantile / _lerp, operation for operation
+// (NaN when the frame has no valid pixel, where the script computes none), then the script's scale.
+__global__ void hs_pick_kernel(int pass, int B, const unsigned long long* __restrict__ counts,
+                               const unsigned int* __restrict__ hist, unsigned long long* __restrict__ sel,
+                               double scale_num, double* __restrict__ stats) {
+  const int b = blockIdx.x, r = threadIdx.x;
+  const unsigned long long n = counts[2 * b], n_nan = counts[2 * b + 1];
+  // (n - 1) * 0.9 in fp64; previous = floor, or -1 (the last element) when at or past n - 1 (n == 1)
+  const double v = __dmul_rn((double)(long long)(n - 1), 0.9);
+  const bool above = v >= (double)(long long)(n - 1);
+  const double prev = above ? -1.0 : floor(v);
+  if (n != 0 && n_nan == 0) {
+    if (pass == 0) {
+      sel[4 * b + r] = 0ull;
+      sel[4 * b + 2 + r] = above ? n - 1 : (unsigned long long)prev + r;
+    }
+    const unsigned int* h = hist + ((long long)pass * B + b) * 512 + r * 256;
+    unsigned long long below = 0, want = sel[4 * b + 2 + r];
+    int dig = 255;
+    for (int j = 0; j < 256; ++j) {
+      if (want < below + h[j]) { dig = j; break; }
+      below += h[j];
+    }
+    sel[4 * b + 2 + r] = want - below;
+    sel[4 * b + r] |= (unsigned long long)dig << (56 - 8 * pass);
+  }
+  __syncthreads();
+  if (pass != kHsPasses - 1 || r != 0) return;
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  double s, p90 = nan;
+  if (n == 0) {
+    s = 1.0;
+  } else {
+    if (n_nan == 0) {
+      const double a = hs_value(sel[4 * b]), c = hs_value(sel[4 * b + 1]);
+      const double gamma = __dsub_rn(v, prev);
+      const double diff = __dsub_rn(c, a);
+      p90 = __dadd_rn(a, __dmul_rn(diff, gamma));
+      if (gamma >= 0.5) p90 = __dsub_rn(c, __dmul_rn(diff, __dsub_rn(1.0, gamma)));
+    }
+    s = p90 < 1e-4 ? 0.0 : __ddiv_rn(scale_num, p90);
+  }
+  stats[2 * b] = p90;
+  stats[2 * b + 1] = s;
+}
+
+// Per pixel: the tone-mapped B, G, R bytes and the uint16 plane depth in millimetres.
+template <typename TR, typename TD>
+__global__ void hs_frame_kernel(const TR* __restrict__ rgb, const TD* __restrict__ dist, const int* __restrict__ eid,
+                                int H, int W, double focal, const double* __restrict__ stats,
+                                unsigned char* __restrict__ bgr, unsigned short* __restrict__ depth) {
+  const int b = blockIdx.y;
+  const long long HW = (long long)H * W;
+  const double s = stats[2 * b + 1];
+  const float ff = __double2float_rn(focal), fz = __fmul_rn(ff, ff);
+  const double x0 = __dadd_rn(-0.5 * W, 0.5), y0 = __dadd_rn(-0.5 * H, 0.5);   // np.linspace's start
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
+    const long long g = (long long)b * HW + i;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const double t = __dmul_rn(s, hs_load(rgb, 3 * g + c));
+      bgr[3 * g + 2 - c] = hs_tone(isnan(t) ? t : (t > 0.0 ? t : 0.0));
+    }
+    // dist_2_depth: the float32 image-plane point (x, y, f), its fp32 norm, then fp64 distance / norm * f
+    const float px = (float)__dadd_rn((double)(i % W), x0), py = (float)__dadd_rn((double)(i / W), y0);
+    const float nrm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), fz));
+    const double d = eid[g] != -1 ? __dmul_rn(__ddiv_rn(hs_load(dist, g), (double)nrm), focal) : 0.0;
+    depth[g] = (unsigned short)trunc_wrap(__dmul_rn(d, 1000.0));
+  }
+}
+
+// p_out[i] = the power hs_tone uses for m = x[i] and level_out[i] its uint8 level
+__global__ void debug_hypersim_pow_kernel(const double* __restrict__ x, long long n, int force_slow,
+                                          double* __restrict__ p_out, unsigned char* __restrict__ level_out,
+                                          unsigned int* __restrict__ slow_count) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    bool slow = false;
+    double p;
+    level_out[i] = hs_tone(x[i], force_slow != 0, &slow, &p);
+    p_out[i] = p;
+    if (slow && slow_count) atomicAdd(slow_count, 1u);
+  }
+}
+
+// workspace: keys [B][HW] | counts [B][2] | sel [B][4] | stats [B][2] (p90, scale) | hist [passes][B][2][256]
+static long long hs_workspace_bytes(int B, long long HW) {
+  return (long long)B * (HW * 8 + 2 * 8 + 4 * 8 + 2 * 8 + kHsPasses * 512 * 4);
+}
+
+template <typename TR, typename TD>
+static int hs_launch(const void* rgb, const void* dist, const int* eid, int B, int H, int W, double focal,
+                     double scale_num, unsigned char* bgr, unsigned short* depth, int* err, double* stats_out,
+                     void* ws, cudaStream_t st) {
+  const long long HW = (long long)H * W;
+  unsigned long long* keys = (unsigned long long*)ws;
+  unsigned long long* counts = keys + (long long)B * HW;
+  unsigned long long* sel = counts + 2 * B;
+  double* stats = (double*)(sel + 4 * B);
+  unsigned int* hist = (unsigned int*)(stats + 2 * B);
+  cudaError_t e = cudaMemsetAsync(counts, 0, (size_t)B * 2 * 8, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(hist, 0, (size_t)B * kHsPasses * 512 * 4, st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(err, 0, (size_t)B * sizeof(int), st);
+  if (e != cudaSuccess) {
+    set_last_error("b200_data_hypersim_frames: memset: %s", cudaGetErrorString(e));
+    return (int)e;
+  }
+  hs_keys_kernel<TR><<<dim3(data_grid(HW), B), kDataThreads, 0, st>>>((const TR*)rgb, eid, HW, keys, counts, err);
+  B200_CHECK_LAUNCH("hs_keys_kernel");
+  const long long ctas = (HW + kHsHistThreads * 16 - 1) / (kHsHistThreads * 16);
+  const unsigned hist_grid = (unsigned)(ctas < 1 ? 1 : (ctas > kHsHistCtas ? kHsHistCtas : ctas));
+  for (int pass = 0; pass < kHsPasses; ++pass) {
+    hs_hist_kernel<<<dim3(hist_grid, B), kHsHistThreads, 0, st>>>(keys, HW, pass, counts, sel, hist);
+    B200_CHECK_LAUNCH("hs_hist_kernel");
+    hs_pick_kernel<<<B, 2, 0, st>>>(pass, B, counts, hist, sel, scale_num, stats);
+    B200_CHECK_LAUNCH("hs_pick_kernel");
+  }
+  hs_frame_kernel<TR, TD><<<dim3(data_grid(HW), B), kDataThreads, 0, st>>>((const TR*)rgb, (const TD*)dist, eid, H, W,
+                                                                          focal, stats, bgr, depth);
+  B200_CHECK_LAUNCH("hs_frame_kernel");
+  if (stats_out) {
+    e = cudaMemcpyAsync(stats_out, stats, (size_t)B * 2 * sizeof(double), cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) {
+      set_last_error("b200_data_hypersim_frames: stats copy: %s", cudaGetErrorString(e));
+      return (int)e;
+    }
+  }
+  return 0;
+}
+
 }  // namespace b200
 
 using namespace b200;
@@ -451,6 +721,49 @@ extern "C" int b200_debug_pow_e32_neg(const float* x, long long n, int force_slo
   B200_CHECK_ARG(n >= 1, "b200_debug_pow_e32_neg: n=%lld", n);
   debug_pow_e32_neg_kernel<<<data_grid(n), kDataThreads, 0, (cudaStream_t)stream>>>(x, n, force_slow, out, slow_count);
   B200_CHECK_LAUNCH("debug_pow_e32_neg_kernel");
+  return 0;
+}
+
+extern "C" long long b200_data_hypersim_workspace_bytes(int B, int H, int W) {
+  return (B >= 1 && H >= 1 && W >= 1) ? hs_workspace_bytes(B, (long long)H * W) : -1;
+}
+
+extern "C" int b200_data_hypersim_frames(const void* rgb, int rgb_half, const void* dist, int dist_half,
+                                         const int* entity_id, int B, int H, int W, double focal, double scale_num,
+                                         unsigned char* bgr, unsigned short* depth_mm, int* error_flag,
+                                         double* stats_out, void* workspace, long long workspace_bytes,
+                                         void* stream) {
+  B200_CHECK_ARG(rgb && dist && entity_id && bgr && depth_mm && error_flag && workspace,
+                 "b200_data_hypersim_frames: null pointer");
+  B200_CHECK_ARG(B >= 1 && B <= 65535 && H >= 1 && W >= 1 && H < (1 << 23) && W < (1 << 23) &&
+                     (long long)H * W < (1LL << 40),
+                 "b200_data_hypersim_frames: bad shape B=%d H=%d W=%d", B, H, W);
+  B200_CHECK_ARG(isfinite(focal) && isfinite((float)focal), "b200_data_hypersim_frames: non-finite focal length");
+  B200_CHECK_ARG(workspace_bytes >= hs_workspace_bytes(B, (long long)H * W),
+                 "b200_data_hypersim_frames: workspace of %lld bytes, need %lld", workspace_bytes,
+                 hs_workspace_bytes(B, (long long)H * W));
+  B200_CHECK_ARG(((uintptr_t)workspace & 7) == 0, "b200_data_hypersim_frames: workspace not 8-byte aligned");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (rgb_half && dist_half)
+    return hs_launch<__half, __half>(rgb, dist, entity_id, B, H, W, focal, scale_num, bgr, depth_mm, error_flag,
+                                     stats_out, workspace, st);
+  if (rgb_half)
+    return hs_launch<__half, float>(rgb, dist, entity_id, B, H, W, focal, scale_num, bgr, depth_mm, error_flag,
+                                    stats_out, workspace, st);
+  if (dist_half)
+    return hs_launch<float, __half>(rgb, dist, entity_id, B, H, W, focal, scale_num, bgr, depth_mm, error_flag,
+                                    stats_out, workspace, st);
+  return hs_launch<float, float>(rgb, dist, entity_id, B, H, W, focal, scale_num, bgr, depth_mm, error_flag, stats_out,
+                                 workspace, st);
+}
+
+extern "C" int b200_debug_hypersim_pow(const double* x, long long n, int force_slow, double* p_out,
+                                       unsigned char* level_out, unsigned int* slow_count, void* stream) {
+  B200_CHECK_ARG(x && p_out && level_out, "b200_debug_hypersim_pow: null pointer");
+  B200_CHECK_ARG(n >= 1, "b200_debug_hypersim_pow: n=%lld", n);
+  debug_hypersim_pow_kernel<<<data_grid(n), kDataThreads, 0, (cudaStream_t)stream>>>(x, n, force_slow, p_out, level_out,
+                                                                                   slow_count);
+  B200_CHECK_LAUNCH("debug_hypersim_pow_kernel");
   return 0;
 }
 

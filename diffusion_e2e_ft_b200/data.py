@@ -7,6 +7,8 @@ transforms on the device (DESIGN.md §3 "Training inputs").
                                  `.to(device)` of the training loop, on a collated batch of one dataset
     vkitti_normals            <- depth-to-normal-translator/python/gen_vkitti_normals.py:97-136 (D2NT v3) on a batch
     generate_vkitti_normals   <- the whole of gen_vkitti_normals.py: vkitti_DAG_normals/ written from the depths
+    hypersim_frames           <- Marigold's hypersim_util.tone_map and dist_2_depth (preprocess_hypersim.py) on a batch
+    preprocess_hypersim       <- the whole of preprocess_hypersim.py: the PNGs, lists and CSVs Hypersim reads
 
 A training loop keeps its DataLoaders and swaps `from dataloaders.load import *` for this module, then calls
 `batch = prepare_batch(batch)` on every batch.  The returned dict has the keys, shapes and dtypes the reference's
@@ -430,16 +432,26 @@ class _VKITTIDepthFrames(VirtualKITTI2):
 
 
 def _equal_size_batches(frames, batch_size):
-    """Consecutive frames of one size, at most batch_size at a time: (paths, uint16 [B,H,W])."""
-    paths, depths = [], []
-    for path, depth in frames:
-        if depths and (len(depths) == batch_size or depth.shape != depths[0].shape):
-            yield paths, torch.stack(depths)
-            paths, depths = [], []
-        paths.append(path)
-        depths.append(depth)
-    if depths:
-        yield paths, torch.stack(depths)
+    """Consecutive frames of one size and dtype, at most batch_size at a time: (keys, stacked [B,...]).  A frame is
+    (key, tensor) or (key, tuple or list of tensors, as a DataLoader hands a tuple back); those are stacked member by
+    member into a tuple, and such frames are of one size when every member's shape and dtype match."""
+    keys, items = [], []
+
+    def shape(x):
+        return tuple((t.shape, t.dtype) for t in x) if isinstance(x, (tuple, list)) else (x.shape, x.dtype)
+
+    def stack():
+        if isinstance(items[0], (tuple, list)):
+            return tuple(torch.stack(m) for m in zip(*items))
+        return torch.stack(items)
+    for key, item in frames:
+        if items and (len(items) == batch_size or shape(item) != shape(items[0])):
+            yield keys, stack()
+            keys, items = [], []
+        keys.append(key)
+        items.append(item)
+    if items:
+        yield keys, stack()
 
 
 def _normals_on_host(depth, dev):
@@ -453,11 +465,34 @@ def _normals_on_host(depth, dev):
     return host.numpy().copy()
 
 
-def _write_png(path, normals):
+def _write_png(path, image):
     import cv2
     os.makedirs(os.path.dirname(path), exist_ok=True)
-    if not cv2.imwrite(path, normals):
+    if not cv2.imwrite(path, image):
         raise OSError(f"cv2.imwrite could not write {path}")
+
+
+def _bounded_writes(pool, jobs, write, max_pending, done=None):
+    """Submit write(*job) to `pool` for each job in turn, with at most max_pending submitted and not yet finished:
+    beyond that the oldest is waited for first.  `jobs` is consumed lazily, so a generator that computes its frames
+    only computes the next batch once the queue has room, and host memory stays bounded however much slower writing is
+    than computing.  Each result goes to done(result) in submission order.  Returns the number of jobs finished."""
+    pending = collections.deque()
+    finished = 0
+
+    def finish():
+        nonlocal finished
+        r = pending.popleft().result()
+        finished += 1
+        if done is not None:
+            done(r)
+    for job in jobs:
+        while len(pending) >= max_pending:
+            finish()
+        pending.append(pool.submit(write, *job))
+    while pending:
+        finish()
+    return finished
 
 
 def generate_vkitti_normals(root_dir, batch_size=8, num_workers=4, device=None):
@@ -477,18 +512,242 @@ def generate_vkitti_normals(root_dir, batch_size=8, num_workers=4, device=None):
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     frames = DataLoader(_VKITTIDepthFrames(root_dir), batch_size=None, shuffle=False, num_workers=num_workers)
-    max_pending = 2 * max(batch_size, num_workers)
+    with torch.cuda.device(dev), ThreadPoolExecutor(max(1, num_workers)) as pool:
+        jobs = ((p, n) for paths, depth in _equal_size_batches(frames, batch_size)
+                for p, n in zip(paths, _normals_on_host(depth, dev)))
+        return _bounded_writes(pool, jobs, _write_png, 2 * max(batch_size, num_workers))
+
+
+# ------------------------------------------------------------------------------------ Hypersim preprocessing
+HYPERSIM_SPLITS = ("train", "val", "test")
+_HYPERSIM_HALF = {torch.float16: 1, torch.float32: 0}
+_TONE_MAP_NUM = None
+
+
+class HypersimEntityIdError(ValueError):
+    """A frame holds render_entity_id 0, which preprocess_hypersim.py asserts against.  `frames` lists the batch
+    positions of the offending frames."""
+
+    def __init__(self, message, frames):
+        super().__init__(message)
+        self.frames = list(frames)
+
+
+def _tone_map_numerator():
+    """hypersim_util.tone_map's np.power(0.8, inv_gamma), inv_gamma = 1.0 / (1.0 / 2.2), correctly rounded."""
+    global _TONE_MAP_NUM
+    if _TONE_MAP_NUM is None:
+        from decimal import Decimal, localcontext
+        with localcontext() as c:
+            c.prec = 60
+            _TONE_MAP_NUM = float((Decimal(1.0 / (1.0 / 2.2)) * Decimal(0.8).ln()).exp())
+    return _TONE_MAP_NUM
+
+
+def _check_hypersim_frames(rgb, dist, entity_id, focal):
+    def desc(t):
+        return f"{t.dtype} {tuple(t.shape)} on {t.device}" if isinstance(t, torch.Tensor) else type(t).__name__
+    for name, t, dts, nd in (("rgb", rgb, _HYPERSIM_HALF, 4), ("dist", dist, _HYPERSIM_HALF, 3),
+                             ("entity_id", entity_id, (torch.int32,), 3)):
+        if not isinstance(t, torch.Tensor) or t.dtype not in dts or t.dim() != nd:
+            raise ValueError(f"hypersim_frames: {name} must be a {nd}-d {' or '.join(map(str, dts))} tensor, "
+                             f"got {desc(t)}")
+        if not t.is_cuda:
+            raise ValueError(f"hypersim_frames runs on a CUDA device (no CPU fallback), got {name} on {t.device}")
+    B, H, W = dist.shape
+    if tuple(rgb.shape) != (B, H, W, 3) or tuple(entity_id.shape) != (B, H, W):
+        raise ValueError(f"hypersim_frames needs rgb [B,H,W,3], dist and entity_id [B,H,W]: got {tuple(rgb.shape)}, "
+                         f"{tuple(dist.shape)}, {tuple(entity_id.shape)}")
+    if not (1 <= B <= 65535 and 1 <= H < 2 ** 23 and 1 <= W < 2 ** 23):
+        raise ValueError(f"hypersim_frames needs 1 <= B <= 65535 and 1 <= H, W < 2^23, got {tuple(dist.shape)}")
+    if rgb.device != dist.device or entity_id.device != dist.device:
+        raise ValueError(f"hypersim_frames: rgb, dist and entity_id on different devices: {rgb.device}, "
+                         f"{dist.device}, {entity_id.device}")
+    focal = float(focal)
+    with np.errstate(over="ignore"):
+        if not (math.isfinite(focal) and np.isfinite(np.float32(focal))):
+            raise ValueError(f"hypersim_frames needs a finite focal length, got {focal}")
+    return focal
+
+
+def hypersim_frames(rgb, dist, entity_id, focal=HYPERSIM_FOCAL):
+    """Tone mapping and plane depth of preprocess_hypersim.py for B frames on the device: radiance rgb [B,H,W,3] and
+    distance-from-camera-centre dist [B,H,W] (float16 or float32, taken exactly to fp64 as the script's
+    astype(float)), render_entity_id [B,H,W] int32 -> (bgr, depth): bgr uint8 [B,H,W,3] is hypersim_util.tone_map
+    times 255, truncated, in the order the script hands cv2.imwrite (B, G, R); depth uint16 [B,H,W] is dist_2_depth
+    in millimetres, 0 where entity id == -1, through NumPy's wrapping cast (plane depths past 65.535 m wrap, as the
+    script's do).  focal is the script's FOCAL_LENGTH; H and W are the tensors' (the script hard-codes 768 x 1024).
+    Bitwise the script's output with its np.power correctly rounded (DESIGN.md §3.12).  Runs under
+    torch.cuda.device(rgb.device) on its current stream.  An entity id of 0, which the script asserts against, raises
+    HypersimEntityIdError (a ValueError) whose `frames` are the offending batch positions; reading that flag back is
+    the call's one host sync.  Bad arguments raise ValueError before any launch."""
+    focal = _check_hypersim_frames(rgb, dist, entity_id, focal)
+    B, H, W = dist.shape
+    with torch.cuda.device(rgb.device):
+        L = _lib.load()
+        rgb_c, dist_c, eid = rgb.contiguous(), dist.contiguous(), entity_id.contiguous()
+        bgr = torch.empty((B, H, W, 3), dtype=torch.uint8, device=rgb.device)
+        depth = torch.empty((B, H, W), dtype=torch.uint16, device=rgb.device)
+        err = torch.empty(B, dtype=torch.int32, device=rgb.device)
+        nbytes = L.b200_data_hypersim_workspace_bytes(B, H, W)
+        ws = torch.empty(nbytes // 8 + 1, dtype=torch.float64, device=rgb.device)
+        _ck(L.b200_data_hypersim_frames(_p(rgb_c), _HYPERSIM_HALF[rgb.dtype], _p(dist_c), _HYPERSIM_HALF[dist.dtype],
+                                        _p(eid), B, H, W, focal, _tone_map_numerator(), _p(bgr), _p(depth), _p(err),
+                                        None, _p(ws), ws.numel() * 8, _stream()), "b200_data_hypersim_frames")
+        bad = torch.nonzero(err.cpu()).flatten().tolist()
+    if bad:
+        raise HypersimEntityIdError(f"hypersim_frames: render_entity_id holds 0 in frame(s) {bad} (the reference "
+                                    "asserts entity_id != 0)", bad)
+    return bgr, depth
+
+
+def _hypersim_paths(row):
+    """preprocess_hypersim.py's input files of one metadata row (color, depth_meters, render_entity_id), relative to
+    the dataset directory."""
+    images = os.path.join(row.scene_name, "images")
+    geo = os.path.join(images, f"scene_{row.camera_name}_geometry_hdf5")
+    return (os.path.join(images, f"scene_{row.camera_name}_final_hdf5", f"frame.{row.frame_id:04d}.color.hdf5"),
+            os.path.join(geo, f"frame.{row.frame_id:04d}.depth_meters.hdf5"),
+            os.path.join(geo, f"frame.{row.frame_id:04d}.render_entity_id.hdf5"))
+
+
+def _import_h5py():
+    try:
+        import h5py
+    except ImportError as e:
+        raise ImportError("preprocess_hypersim reads Hypersim's HDF5 renders with h5py: `pip install h5py`") from e
+    return h5py
+
+
+class _HypersimRawFrames(Dataset):
+    """One split's frames as (metadata index, (rgb, dist, entity_id)) host tensors in the files' dtypes; decoded with
+    h5py in DataLoader workers."""
+
+    def __init__(self, dataset_dir, rows):
+        self.dataset_dir = dataset_dir
+        self.rows = rows                           # [(index, (color, depth_meters, render_entity_id) paths)]
+
+    def __len__(self):
+        return len(self.rows)
+
+    def __getitem__(self, idx):
+        h5py = _import_h5py()
+        i, paths = self.rows[idx]
+        arrays = []
+        for path, dts in zip(paths, (("float16", "float32"), ("float16", "float32"), ("int32",))):
+            full = os.path.join(self.dataset_dir, path)
+            with h5py.File(full, "r") as f:
+                a = np.array(f["dataset"])
+            if a.dtype.name not in dts:
+                raise ValueError(f"{full}: expected {' or '.join(dts)} data, got {a.dtype}")
+            arrays.append(torch.from_numpy(np.ascontiguousarray(a)))
+        return i, tuple(arrays)
+
+
+def _hypersim_on_host(rgb, dist, entity_id, focal, dev):
+    """One batch of host tensors -> (bgr uint8 [B,H,W,3], depth uint16 [B,H,W]) as numpy arrays in ordinary host
+    memory, computed on `dev` (the staging buffers are released on return, as in _normals_on_host)."""
+    bgr, depth = hypersim_frames(*(t.pin_memory().to(dev, non_blocking=True) for t in (rgb, dist, entity_id)), focal)
+    host = [torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for t in (bgr, depth)]
+    for h, t in zip(host, (bgr, depth)):
+        h.copy_(t, non_blocking=True)
+    torch.cuda.current_stream().synchronize()
+    return tuple(h.numpy().copy() for h in host)
+
+
+def _write_hypersim_frame(split_output_dir, i, rgb_path, depth_path, bgr, depth, valid_mask):
+    """The PNG writes and the metadata of one frame, computed with the script's own NumPy calls on the same uint8 RGB
+    and uint16 depth arrays."""
+    _write_png(os.path.join(split_output_dir, rgb_path), bgr)
+    _write_png(os.path.join(split_output_dir, depth_path), depth)
+    rgb_int = np.ascontiguousarray(bgr[..., ::-1])
+    restored_depth = depth / 1000.0
+    invalid_ratio = (np.prod(valid_mask.shape) - valid_mask.sum()) / np.prod(valid_mask.shape)
+    return i, {"rgb_path": rgb_path, "rgb_mean": np.mean(rgb_int), "rgb_std": np.std(rgb_int),
+               "rgb_min": np.min(rgb_int), "rgb_max": np.max(rgb_int), "depth_path": depth_path,
+               "depth_mean": np.mean(restored_depth), "depth_std": np.std(restored_depth),
+               "depth_min": np.min(restored_depth), "depth_max": np.max(restored_depth),
+               "invalid_ratio": invalid_ratio}
+
+
+def preprocess_hypersim(split_csv, dataset_dir, output_dir, batch_size=8, num_workers=4, device=None):
+    """What `python preprocess_hypersim.py --split_csv .. --dataset_dir .. --output_dir ..` does, on the device: for
+    every included_in_public_release row of split_csv, split by split (train, val, test), the tone-mapped
+    rgb_{camera}_fr{frame}.png and the 16-bit depth_plane_{camera}_fr{frame}.png under output_dir/{split}/{scene}/,
+    then filename_list_{split}.txt and filename_meta_{split}.csv, byte for byte the script's files (with its
+    np.power correctly rounded).  data.Hypersim reads output_dir as its root_dir.  DataLoader workers read the HDF5
+    files with h5py, batches of up to batch_size frames go through hypersim_frames, and a pool of num_workers threads
+    encodes, writes and computes each frame's metadata, with at most 2 * max(batch_size, num_workers) computed frames
+    waiting at any time.  Returns the number of frames written.
+
+    At the edges: an existing output_dir/{split} raises FileExistsError, as the script's os.makedirs does, but for
+    all three splits before anything is written; a missing input file raises FileNotFoundError naming it (the script
+    fails an assert), also before anything is written; an entity id of 0 raises ValueError naming the file (the
+    script fails an assert); a split without rows gets an empty filename_list and a header-only CSV, where the script
+    stops with an AttributeError."""
+    import pandas as pd
+    if batch_size < 1 or num_workers < 0:
+        raise ValueError(f"need batch_size >= 1 and num_workers >= 0, got {batch_size}, {num_workers}")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device()) \
+        if torch.cuda.is_available() else None
+    if dev is None or dev.type != "cuda":
+        raise ValueError(f"preprocess_hypersim runs on a CUDA device (no CPU fallback), got {dev}")
+    if dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    raw_meta_df = pd.read_csv(split_csv)
+    meta_df = raw_meta_df[raw_meta_df.included_in_public_release].copy()
+    for split in HYPERSIM_SPLITS:
+        if os.path.exists(os.path.join(output_dir, split)):
+            raise FileExistsError(f"{os.path.join(output_dir, split)} exists")
+    plan = []
+    for split in HYPERSIM_SPLITS:
+        split_meta_df = meta_df[meta_df.split_partition_name == split].copy()
+        rows = [(i, _hypersim_paths(row)) for i, row in split_meta_df.iterrows()]
+        for _, paths in rows:
+            for p in paths:
+                if not os.path.exists(os.path.join(dataset_dir, p)):
+                    raise FileNotFoundError(f"{os.path.join(dataset_dir, p)}: input file missing")
+        plan.append((split, split_meta_df, rows))
+    if any(rows for _, _, rows in plan):
+        _import_h5py()
     written = 0
     with torch.cuda.device(dev), ThreadPoolExecutor(max(1, num_workers)) as pool:
-        pending = collections.deque()
-        for paths, depth in _equal_size_batches(frames, batch_size):
-            normals = _normals_on_host(depth, dev)
-            for p, n in zip(paths, normals):
-                while len(pending) >= max_pending:
-                    pending.popleft().result()
-                    written += 1
-                pending.append(pool.submit(_write_png, p, n))
-        while pending:
-            pending.popleft().result()
-            written += 1
+        for split, split_meta_df, rows in plan:
+            split_output_dir = os.path.join(output_dir, split)
+            os.makedirs(split_output_dir)
+            split_meta_df["rgb_path"] = None
+            for col in ("rgb_mean", "rgb_std", "rgb_min", "rgb_max"):
+                split_meta_df[col] = np.nan
+            split_meta_df["depth_path"] = None
+            for col in ("depth_mean", "depth_std", "depth_min", "depth_max", "invalid_ratio"):
+                split_meta_df[col] = np.nan
+            frames = DataLoader(_HypersimRawFrames(dataset_dir, rows), batch_size=None, shuffle=False,
+                                num_workers=num_workers)
+            paths = dict(rows)
+            names = {i: (os.path.join(row.scene_name, f"rgb_{row.camera_name}_fr{row.frame_id:04d}.png"),
+                         os.path.join(row.scene_name, f"depth_plane_{row.camera_name}_fr{row.frame_id:04d}.png"))
+                     for i, row in split_meta_df.iterrows()}
+
+            def jobs():
+                for idx, (rgb, dist, eid) in _equal_size_batches(frames, batch_size):
+                    try:
+                        bgr, depth = _hypersim_on_host(rgb, dist, eid, HYPERSIM_FOCAL, dev)
+                    except HypersimEntityIdError as e:
+                        bad = [os.path.join(dataset_dir, paths[idx[k]][2]) for k in e.frames]
+                        raise HypersimEntityIdError(f"render_entity_id holds 0 in {bad} (the reference asserts "
+                                                    "entity_id != 0)", e.frames) from e
+                    for i, b, d, e in zip(idx, bgr, depth, eid.numpy()):
+                        yield (split_output_dir, i, *names[i], b, d, e != -1)
+
+            def record(result):
+                i, meta = result
+                for k, v in meta.items():
+                    split_meta_df.at[i, k] = v
+            written += _bounded_writes(pool, jobs(), _write_hypersim_frame, 2 * max(batch_size, num_workers), record)
+            with open(os.path.join(split_output_dir, f"filename_list_{split}.txt"), "w+") as f:
+                if len(split_meta_df):
+                    lines = split_meta_df.apply(lambda r: f"{r['rgb_path']} {r['depth_path']}", axis=1).tolist()
+                    f.writelines("\n".join(lines))
+            with open(os.path.join(split_output_dir, f"filename_meta_{split}.csv"), "w+") as f:
+                split_meta_df.to_csv(f, header=True)
     return written

@@ -11,7 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200_e2eft.so")
 
 _lib = None
-ABI_VERSION = 16       # bumped with every signature change of include/b200_e2eft.h
+ABI_VERSION = 17       # bumped with every signature change of include/b200_e2eft.h
 
 _P = c_void_p
 _LL = c_longlong
@@ -114,6 +114,10 @@ _SIGS = {
                                    _P, _P, _P, _P, _P, _P, _P, _P]),
     "b200_data_vkitti_normals": (c_int, [_P, c_int, c_int, c_int, c_float, c_float, c_float, c_float, _P, _P]),
     "b200_debug_pow_e32_neg": (c_int, [_P, _LL, c_int, _P, _P, _P]),
+    "b200_data_hypersim_workspace_bytes": (_LL, [c_int, c_int, c_int]),
+    "b200_data_hypersim_frames": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_double, c_double, _P, _P, _P,
+                                          _P, _P, _LL, _P]),
+    "b200_debug_hypersim_pow": (c_int, [_P, _LL, c_int, _P, _P, _P, _P]),
 }
 EXPORTS = tuple(_SIGS)
 

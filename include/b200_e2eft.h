@@ -521,6 +521,29 @@ int b200_data_vkitti_normals(const unsigned short* depth_cm, int B, int H, int W
 int b200_debug_pow_e32_neg(const float* x, long long n, int force_slow, float* out, unsigned int* slow_count,
                            void* stream);
 
+/* Hypersim preprocessing (ABI 17): Marigold's script/dataset_preprocess/hypersim/preprocess_hypersim.py per frame,
+ * for B frames of radiance rgb [B][H][W][3] and distance dist [B][H][W] (fp32, or fp16 where *_half != 0; both taken
+ * exactly to fp64 as the script's astype(float)) and render_entity_id [B][H][W] int32.  bgr [B][H][W][3] uint8 = the
+ * tone-mapped colour in the order cv2.imwrite takes after the script's cvtColor(RGB2BGR); depth_mm [B][H][W] uint16 =
+ * the plane depth (distance / ||(x, y, focal)||_fp32 * focal) times 1000, 0 where entity id == -1, through NumPy's
+ * wrapping float64 -> uint16 cast.  scale_num is the tone map's pow(0.8, 1 / (1 / 2.2)), computed on the host.
+ * error_flag[b] (int32 [B], device) is set nonzero where frame b holds an entity id of 0, which the script asserts
+ * against.  stats_out (device, nullable) receives [B][2] fp64 per frame: the 90th-percentile brightness (NaN when
+ * the frame has no valid pixel) and the tone map's scale.  Bitwise the script's output with its np.power correctly
+ * rounded (DESIGN.md §3.12).  workspace is device memory of at least b200_data_hypersim_workspace_bytes(B, H, W)
+ * bytes, 8-byte aligned.  Nothing syncs the host. */
+long long b200_data_hypersim_workspace_bytes(int B, int H, int W);
+int b200_data_hypersim_frames(const void* rgb, int rgb_half, const void* dist, int dist_half, const int* entity_id,
+                              int B, int H, int W, double focal, double scale_num, unsigned char* bgr,
+                              unsigned short* depth_mm, int* error_flag, double* stats_out, void* workspace,
+                              long long workspace_bytes, void* stream);
+/* The tone map's power on its own, for testing the correct rounding: for m = x[i] (fp64 [n], the clamped scale * x),
+ * p_out[i] = the pow(m, 1 / 2.2) b200_data_hypersim_frames uses (the correctly rounded value wherever it decides the
+ * level) and level_out[i] = its uint8 level; force_slow != 0 takes the double-double path for every finite m > 0;
+ * slow_count (device, nullable, not reset) is incremented once per element that took it. */
+int b200_debug_hypersim_pow(const double* x, long long n, int force_slow, double* p_out, unsigned char* level_out,
+                            unsigned int* slow_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
