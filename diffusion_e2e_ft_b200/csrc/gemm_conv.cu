@@ -237,6 +237,8 @@ extern "C" int b200_linear(const void* A, long long lda, long long a_batch_strid
                  "b200_linear: pointers must be 16-byte aligned");
   B200_CHECK_ARG(act != ACT_GEGLU || ldo % 8 == 0, "b200_linear: GEGLU needs ldo %% 8 == 0");
   B200_CHECK_ARG(act != ACT_GEGLU || (N % 16 == 0 && bias), "b200_linear: GEGLU needs bias and N%%16==0");
+  // the GEGLU epilogue adds the bias to the raw accumulators of both halves: it has no alpha to apply
+  B200_CHECK_ARG(act != ACT_GEGLU || alpha == 1.0f, "b200_linear: GEGLU needs alpha == 1 (got %g)", (double)alpha);
   B200_CHECK_ARG(batch == 1 || (a_batch_stride % 8 == 0 && (w_batch_stride % 8 == 0)),
                  "b200_linear: batch strides must be multiples of 8 elements");
 

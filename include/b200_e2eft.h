@@ -30,7 +30,7 @@ int b200_abi_version(void);
 /* epilogue activations */
 #define B200_ACT_NONE 0
 #define B200_ACT_SILU 1
-#define B200_ACT_GEGLU 2 /* W rows pre-interleaved per tile: [value half | gate half] */
+#define B200_ACT_GEGLU 2 /* W rows pre-interleaved per tile: [value half | gate half]; alpha must be 1 */
 #define B200_ACT_GELU 3  /* erf GELU */
 #define B200_ACT_EXP2 4  /* exp2(alpha * acc + bias): softmax probabilities recomputed from the log-sum-exp */
 
@@ -284,7 +284,8 @@ int b200_adamw_step_state_groups(float* param, const float* grad, float* exp_avg
  * GroupNorm backward (diffusers GroupNorm(32) + optional SiLU, NHWC): mean_rstd [NB][groups][2] from the
  *   forward's statistics; pass 1 accumulates S [NB][Ctot][2] = (sum dz, sum dz*xhat) per channel (zeroed by
  *   the caller; call once per concatenated input with its channel offset), pass 2 writes
- *   dx = rstd*(dz*gamma - mean_g(gamma dz) - xhat*mean_g(gamma dz xhat)) (+ add).  d_gamma = sum_n S[..1],
+ *   dx = rstd*(dz*gamma - mean_g(gamma dz) - xhat*mean_g(gamma dz xhat)) (+ add), reading S over every group the
+ *   channels [c_off, c_off+Cx) touch (a group straddling c_off includes channels of the other input).  d_gamma = sum_n S[..1],
  *   d_beta = sum_n S[..0].  dy is fp16 [NB][HW][Ctot].
  * b200_layer_norm_bwd: dx (+ add) and d_gamma/d_beta (accumulated into zeroed fp32 [C]).
  * b200_softmax_bwd_rows: dS = scale * P o (dP - rowsum(dP o P)), P/dS fp16, dP fp32.
