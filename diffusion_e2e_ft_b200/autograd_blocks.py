@@ -276,23 +276,11 @@ class _TransformerFn(torch.autograd.Function):
         # ---- self attention: h1 = h0 + W_o1 attn(q, k, v) + b_o1
         do1, g["wo1"], g["bo1"] = bw.linear_bwd(o.view(B * L, C), bp["wo1"], ops.cast_f16(dh1), need_dw=train)
         dqkv = torch.empty((B, L, 3 * C), dtype=F16, device=dev)
-        if not blk.joint:
-            bw.attention_bwd(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], do1.view(B, L, C), heads, scale,
-                             outs=(dqkv[..., :C], dqkv[..., C:2 * C], dqkv[..., 2 * C:]))
-        else:
-            # XFormersJointAttnProcessor (attention.py:430-513): images i and i + B/2 (the depth / normal halves) both
-            # attend to the concatenation of their two key/value sets.  Their queries therefore form ONE attention
-            # problem with 2L queries over 2L keys, whose dK/dV rows are exactly the two images' own gradients.
-            half = B // 2
-            do1 = do1.view(B, L, C)
-            for i in range(half):
-                pair = torch.cat([qkv[i], qkv[i + half]], dim=0).unsqueeze(0)          # [1, 2L, 3C] (host re-layout)
-                dop = torch.cat([do1[i], do1[i + half]], dim=0).unsqueeze(0)
-                dpair = torch.empty((1, 2 * L, 3 * C), dtype=F16, device=dev)
-                bw.attention_bwd(pair[..., :C], pair[..., C:2 * C], pair[..., 2 * C:], dop, heads, scale,
-                                 outs=(dpair[..., :C], dpair[..., C:2 * C], dpair[..., 2 * C:]))
-                dqkv[i].copy_(dpair[0, :L])
-                dqkv[i + half].copy_(dpair[0, L:])
+        # joint blocks (XFormersJointAttnProcessor, attention.py:430-513): images i and i + B/2 attend to the keys of
+        # both, kv_segments = 2 as in the forward
+        bw.attention_bwd(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], do1.view(B, L, C), heads, scale,
+                         outs=(dqkv[..., :C], dqkv[..., C:2 * C], dqkv[..., 2 * C:]),
+                         kv_segments=2 if blk.joint else 1)
         dn1, dwqkv, _ = bw.linear_bwd(n1, bp["wqkv"], dqkv.view(B * L, 3 * C), need_dw=train, bias=False)
         if train:
             g["wq1"], g["wk1"], g["wv1"] = dwqkv[:C], dwqkv[C:2 * C], dwqkv[2 * C:]

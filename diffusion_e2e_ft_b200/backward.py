@@ -192,24 +192,25 @@ def conv_dgrad(dy, w, cin, kind="s1", out_dtype=F32, add=None, packed=None, in_h
 
 
 # --------------------------------------------------------------------------------------------- attention
-def attention_bwd(q, k, v, do, heads, scale, outs=None):
+def attention_bwd(q, k, v, do, heads, scale, outs=None, kv_segments=1):
     """Backward of softmax(scale * q k^T) v per head of width D = C / heads in ops.HEAD_DIMS.  q/do [B,T,C],
-    k/v [B,Tk,C] fp16 views (last dim contiguous).  Returns fp16 (dq, dk, dv) — written into `outs` (row-strided views, e.g. the three
-    column blocks of a fused d(qkv) buffer) when given.
+    k/v [B,Tk,C] fp16 views (last dim contiguous).  Returns fp16 (dq, dk, dv) — written into `outs` (row-strided
+    views, e.g. the three column blocks of a fused d(qkv) buffer) when given.  `kv_segments` = 2: GeoWizard's joint
+    attention (batch b attends to the keys of b % (B/2) and b % (B/2) + B/2, as in ops.attention).
 
-    Round 2: no fp32 score matrices and no softmax passes.  The flash kernel is re-run for (O, log-sum-exp); then per
-    image, batched over heads,
-        P  = exp2(c * Q K^T - lse)                     GEMM with an exp2 epilogue (row bias -lse), fp16 out
-        dS = scale * P o (dO V^T - delta)              GEMM with a row bias (-scale * delta) and P as multiplicative operand
-        dQ = dS K,  dK = dS^T Q,  dV = P^T dO          row contractions, operands consumed MN-major as stored
-    with delta_t = sum_d dO_td O_td (`rowdot_heads`).  Round 1 materialised S and dP in fp32, ran a row softmax and its
-    backward over them and transposed dS / P / Q / K / dO with a gather kernel.
-    Still materialises P and dS ([heads, T, Tk] fp16 per image): a fused flash backward would remove those too."""
+    The flash kernel is re-run for (O, log-sum-exp) and delta_t = sum_d dO_td O_td (`rowdot_heads_d`); then, per head,
+        P  = exp2(c * Q K^T - lse),  dS = scale * P o (dO V^T - delta)
+        dQ = dS K,  dK = dS^T Q,  dV = P^T dO
+    in the fused kernels (ops.attention_bwd): P and dS never leave the SM, so memory is O(B T C) at any length.
+    Tensors the engine's kernels cannot take (not on a CUDA device) go to `_attention_bwd_gemm` instead, the per-image
+    composition of GEMM launches that the fused kernels replaced: its ops raise for such tensors as every op does,
+    and the CPU tests that restate each kernel in plain torch (tests/cpu_emulation.py) check this host algebra
+    through it."""
     B, T, C = q.shape
     Tk = k.shape[1]
     D = C // heads
     assert C == heads * D and D in ops.HEAD_DIMS, (C, heads)
-    Tkp = ops._ru8(Tk)
+    assert kv_segments in (1, 2) and (kv_segments == 1 or B % 2 == 0), (kv_segments, B)
     dev = q.device
     if outs is not None:
         dq, dk, dv = outs
@@ -219,7 +220,7 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
         dk = torch.empty((B, Tk, C), dtype=F16, device=dev)
         dv = torch.empty((B, Tk, C), dtype=F16, device=dev)
 
-    if Tk == 1:
+    if Tk == 1 and kv_segments == 1:
         # One key (GeoWizard's single image-embedding token): the softmax is constant, P = 1, so dS = P o (dP - delta)
         # is exactly zero, as torch.autograd finds it in the reference.  dQ = dK = 0 and dV = the sum of dO over the
         # queries.  The general path would form dP - delta from two differently ordered fp32 sums and leave rounding
@@ -230,19 +231,49 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
             dv[b, 0].copy_(ops.cast_f16(ops.col_sum(do[b])))
         return dq, dk, dv
 
+    o, lse = ops.attention(q, k, v, heads, scale, kv_segments=kv_segments, want_lse=True)   # lse: log2 domain
+    delta = ops.rowdot_heads_d(do, o, heads, D)                                           # [B,heads,T]
+    if q.is_cuda:
+        ops.attention_bwd(q, k, v, do, lse, delta, dq, dk, dv, heads, scale, kv_segments)
+    else:
+        _attention_bwd_gemm(q, k, v, do, heads, scale, lse, delta, dq, dk, dv, kv_segments)
+    return dq, dk, dv
+
+
+def _attention_bwd_gemm(q, k, v, do, heads, scale, lse, delta, dq, dk, dv, kv_segments=1):
+    """The backward as GEMM launches per image, batched over heads, with P and dS stored ([heads, T, Tk] fp16):
+        P  = exp2(c * Q K^T - lse)                     exp2 epilogue with the row bias -lse
+        dS = scale * P o (dO V^T - delta)              row bias -scale * delta, P as multiplicative operand
+        dQ = dS K,  dK = dS^T Q,  dV = P^T dO          row contractions, operands consumed MN-major as stored.
+    Joint attention (kv_segments = 2): the images i and i + B/2 of a pair form one problem of 2T queries over 2Tk keys
+    whose dK / dV rows are the two images' own gradients."""
+    B, T, C = q.shape
+    Tk = k.shape[1]
+    D = C // heads
+    if kv_segments == 2:
+        h = B // 2
+        for i in range(h):
+            pair = lambda t: torch.cat([t[i], t[i + h]], 0).unsqueeze(0)                    # host re-layout
+            g = [torch.empty((1, 2 * L, C), dtype=F16, device=q.device) for L in (T, Tk, Tk)]
+            _attention_bwd_gemm(pair(q), pair(k), pair(v), pair(do), heads, scale, pair(lse.transpose(1, 2)).transpose(
+                1, 2).contiguous(), pair(delta.transpose(1, 2)).transpose(1, 2).contiguous(), *g)
+            for out, gp, L in ((dq, g[0], T), (dk, g[1], Tk), (dv, g[2], Tk)):
+                out[i].copy_(gp[0, :L])
+                out[i + h].copy_(gp[0, L:])
+        return
+    Tkp = ops._ru8(Tk)
+
     def heads_view(t2d):                      # [L, heads*D] -> [heads, L, D] strided view
         return t2d.unflatten(-1, (heads, D)).permute(1, 0, 2)
 
-    o, lse = ops.attention(q, k, v, heads, scale, want_lse=True)             # [B,T,C], [B,heads,T] (log2 domain)
-    delta = ops.rowdot_heads_d(do, o, heads, D)                              # [B,heads,T]
     neg_lse = _scaled(lse, -1.0)
     neg_delta = _scaled(delta, -float(scale))
     c = float(scale) * 1.4426950408889634
     for b in range(B):
         qh, kh, vh, doh = heads_view(q[b]), heads_view(k[b]), heads_view(v[b]), heads_view(do[b])
-        p = torch.empty((heads, T, Tkp), dtype=F16, device=dev)
+        p = torch.empty((heads, T, Tkp), dtype=F16, device=q.device)
         ops.linear(qh, kh, bias=neg_lse[b], bias_row=True, act=ops.ACT_EXP2, alpha=c, out=p[:, :, :Tk])
-        ds = torch.empty((heads, T, Tkp), dtype=F16, device=dev)
+        ds = torch.empty((heads, T, Tkp), dtype=F16, device=q.device)
         ops.linear(doh, vh, bias=neg_delta[b], bias_row=True, alpha=float(scale), residual=p[:, :, :Tk], res_mul=True,
                    out=ds[:, :, :Tk])
         # dQ[h] = dS[h] @ K[h]            (K [Tk, D] = [contraction, columns])
@@ -250,7 +281,6 @@ def attention_bwd(q, k, v, do, heads, scale, outs=None):
         # dK[h] = dS[h]^T @ Q[h], dV[h] = P[h]^T @ dO[h]   (contraction over the T query rows of both operands)
         ops.linear(ds[:, :, :Tk], qh, out=heads_view(dk[b]), a_t=True, w_t=True)
         ops.linear(p[:, :, :Tk], doh, out=heads_view(dv[b]), a_t=True, w_t=True)
-    return dq, dk, dv
 
 
 def _scaled(t, f):

@@ -21,8 +21,7 @@
 //   D = 40, 64   3 warpgroups, 128-key tiles, 3 stages   (Q 24 KB + K/V 96 KB; S 64 + P 32 + O <= 32 registers)
 //   D = 80       3 warpgroups,  64-key tiles, 3 stages   (Q 48 KB + K/V 96 KB; 128-key tiles spill at 128 registers)
 //   D = 160      2 warpgroups,  64-key tiles, 3 stages   (Q 48 KB + K/V 144 KB; O 80 + S 32 + P 16 registers)
-#include "common.cuh"
-#include "wgmma.cuh"
+#include "attention.cuh"
 #include "../../include/b200_e2eft.h"
 
 namespace b200 {
@@ -58,31 +57,6 @@ struct AttParams {
   long long o_bs, o_ls;
   float* lse;                  // optional [B][heads][Lq]: log2-domain log-sum-exp of the scaled scores (backward pass)
 };
-
-__device__ __forceinline__ float ex2_approx(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-  uint32_t r;
-  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));   // low half = a, high half = b
-  return r;
-}
-
-template <int BK>
-__device__ __forceinline__ void wgmma_qk(float* s, uint64_t da, uint64_t db, int scale_d) {
-  if constexpr (BK == 128) wgmma_m64n128<0, 0>(s, da, db, scale_d);
-  else wgmma_m64n64<0, 0>(s, da, db, scale_d);
-}
-
-template <int D>
-__device__ __forceinline__ void wgmma_pv(float* o, const uint32_t (&a)[4], uint64_t db) {
-  if constexpr (D == 40) wgmma_m64n40_rs_bmn(o, a, db);
-  else if constexpr (D == 64) wgmma_m64n64_rs_bmn(o, a, db);
-  else if constexpr (D == 80) wgmma_m64n80_rs_bmn(o, a, db);
-  else wgmma_m64n160_rs_bmn(o, a, db);
-}
 
 template <int D>
 __global__ void __launch_bounds__(AttShape<D>::kThreads, 1)
@@ -180,8 +154,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       wgmma_fence();
 #pragma unroll
       for (int k = 0; k < S_::kKSteps; ++k)        // k-step k: columns 16 (k % 4) .. of atom k / 4 (+32 B per step)
-        wgmma_qk<kBk>(s, qdesc + (k / 4) * (S_::kQAtom >> 4) + 2 * (k % 4),
-                      kdesc + (k / 4) * (S_::kKvAtom >> 4) + 2 * (k % 4), k != 0);
+        wgmma_ss<kBk>(s, kstep_desc(qdesc, k, S_::kQAtom), kstep_desc(kdesc, k, S_::kKvAtom), k != 0);
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_operands<kBk / 2>(s);
@@ -244,7 +217,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kBk / 16; ++kk)       // B = V[16 kk .. 16 kk + 15, :]: MN-major, 2 groups of 8 key rows
-        wgmma_pv<D>(o, pa[kk], make_desc_sw128(vbase + kk * 2048, S_::kKvAtom, 1024));   // atoms kKvAtom apart
+        wgmma_rs_d<D>(o, pa[kk], make_desc_sw128(vbase + kk * 2048, S_::kKvAtom, 1024));   // atoms kKvAtom apart
       wgmma_commit();
       wgmma_wait<0>();
       wgmma_fence_operands<D / 2>(o);
@@ -494,25 +467,11 @@ template <int D>
 int launch_attention(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs, long long k_ls,
                      const void* v, long long v_bs, long long v_ls, const AttParams& p, void* stream) {
   using S_ = AttShape<D>;
-  // {D, heads, L, B}: one head is the innermost dimension, so a 64-column box past D reads zeros, not the next head
   CUtensorMap tq, tk, tv;
-  const uint32_t box[4] = {64, 1, kBq, 1};
-  const uint32_t kv_box[4] = {64, 1, S_::kBk, 1};
-  {
-    uint64_t dims[4] = {(uint64_t)D, (uint64_t)p.heads, (uint64_t)p.Lq, (uint64_t)p.B};
-    uint64_t str[3] = {(uint64_t)D * 2, (uint64_t)q_ls * 2, (uint64_t)q_bs * 2};
-    int r = encode_tmap(&tq, q, 4, dims, str, box, nullptr);
-    if (r) return r;
-  }
-  {
-    uint64_t dims[4] = {(uint64_t)D, (uint64_t)p.heads, (uint64_t)p.Lk, (uint64_t)p.B};
-    uint64_t str[3] = {(uint64_t)D * 2, (uint64_t)k_ls * 2, (uint64_t)k_bs * 2};
-    int r = encode_tmap(&tk, k, 4, dims, str, kv_box, nullptr);
-    if (r) return r;
-    uint64_t strv[3] = {(uint64_t)D * 2, (uint64_t)v_ls * 2, (uint64_t)v_bs * 2};
-    r = encode_tmap(&tv, v, 4, dims, strv, kv_box, nullptr);
-    if (r) return r;
-  }
+  int r = encode_head_tmap(&tq, q, D, p.heads, p.Lq, p.B, q_ls, q_bs, kBq);
+  if (!r) r = encode_head_tmap(&tk, k, D, p.heads, p.Lk, p.B, k_ls, k_bs, S_::kBk);
+  if (!r) r = encode_head_tmap(&tv, v, D, p.heads, p.Lk, p.B, v_ls, v_bs, S_::kBk);
+  if (r) return r;
   static bool configured_dev[kMaxDevices] = {false};      // per device: function attributes live in the context
   const int dev_ = current_device();
   bool& configured = configured_dev[dev_ < 0 ? 0 : dev_];

@@ -120,6 +120,12 @@ _SIGS = {
     "b200_debug_hypersim_pow": (c_int, [_P, _LL, c_int, _P, _P, _P, _P]),
 }
 EXPORTS = tuple(_SIGS)
+# the fused attention backward, declared in include/b200_e2eft_attention_bwd.h
+_SIGS_ATTENTION_BWD = {
+    "b200_attention_bwd": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _P, _P, _LL, _LL,
+                                   _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
+                                   _P]),
+}
 
 
 def load(build_if_missing=True):
@@ -139,7 +145,7 @@ def load(build_if_missing=True):
     if lib.b200_abi_version() != ABI_VERSION:
         raise RuntimeError(f"{LIB_PATH} exports ABI {lib.b200_abi_version()}, this package binds ABI {ABI_VERSION}: "
                            "rebuild with `python -m diffusion_e2e_ft_b200.build --force`")
-    for name, (res, args) in _SIGS.items():
+    for name, (res, args) in {**_SIGS, **_SIGS_ATTENTION_BWD}.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

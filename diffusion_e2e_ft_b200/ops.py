@@ -362,6 +362,34 @@ def _attention(q, k, v, heads, D, scale, kv_segments, out, want_lse):
     return (out, lse) if want_lse else out
 
 
+def _bstride(t, L):
+    """Batch stride of a [B, L, C] view as the kernels take it (a single batch element may have any stride(0))."""
+    return t.stride(0) if t.shape[0] > 1 else t.stride(1) * L
+
+
+@_timed("attention_bwd")
+def attention_bwd(q, k, v, do, lse, delta, dq, dk, dv, heads, scale, kv_segments=1):
+    """Fused flash attention backward (b200_attention_bwd): q / do / dq [B,Lq,C], k / v / dk / dv [B,Lk,C] fp16 views
+    (last dim contiguous, e.g. column blocks of fused QKV / d(QKV) buffers), lse / delta fp32 [B, heads, Lq] from
+    `attention(..., want_lse=True)` and `rowdot_heads_d(do, out, ...)`.  Writes dq, dk, dv; P and dS stay on chip."""
+    _need_cuda(q, k, v, do, dq, dk, dv)
+    C = q.shape[-1]
+    D = C // heads
+    B, Lq, Lk = q.shape[0], q.shape[1], k.shape[1]
+    for t in (q, k, v, do, dq, dk, dv):
+        assert t.dtype == F16 and t.stride(-1) == 1 and t.shape[-1] == C, (t.dtype, t.shape, t.stride())
+    assert lse.dtype == F32 and delta.dtype == F32 and lse.is_contiguous() and delta.is_contiguous()
+    assert tuple(lse.shape) == (B, heads, Lq) and tuple(delta.shape) == (B, heads, Lq)
+    rc = _lib.load().b200_attention_bwd(
+        _p(q), _bstride(q, Lq), q.stride(1), _p(k), _bstride(k, Lk), k.stride(1), _p(v), _bstride(v, Lk), v.stride(1),
+        _p(do), _bstride(do, Lq), do.stride(1), _p(lse), _p(delta), _p(dq), _bstride(dq, Lq), dq.stride(1),
+        _p(dk), _bstride(dk, Lk), dk.stride(1), _p(dv), _bstride(dv, Lk), dv.stride(1),
+        B, heads, D, Lq, Lk, kv_segments, float(scale), _stream())
+    _lib.check(rc, "b200_attention_bwd")
+    STATS.add("attn", 10 * B * heads * Lq * Lk * kv_segments * D)       # the 5 products of the backward
+    return dq, dk, dv
+
+
 @_timed("attention")
 def attention_d512(q, k, v, scale, out=None):
     """One head of width 512 (VAE mid-block): q [B,Lq,512], k/v [B,Lk,512] fp16 views (last dim contiguous, e.g.

@@ -144,7 +144,9 @@ class B200UNet2DConditionModel(PretrainedMixin, nn.Module):
         return next(self.parameters()).device
 
     def enable_xformers_memory_efficient_attention(self, *a, **k):
-        """No-op: the engine's attention is always the fused flash kernel (Marigold/run.py:284-287)."""
+        """No-op: the engine's attention always runs memory-efficiently (Marigold/run.py:284-287): the forward is the
+        flash kernel, and the training backward recomputes P and dS on chip in the fused backward kernels, so neither
+        pass stores a [heads, T, Tk] matrix."""
 
     def enable_gradient_checkpointing(self):
         self._gradient_checkpointing = True
