@@ -423,29 +423,53 @@ def embed(unet, t, class_labels):
 
 # ------------------------------------------------------------------------------------ VAE mid-block attention
 class _VAEAttentionFn(torch.autograd.Function):
-    """VAEAttention's unfused path (single head, d = channels) + its data gradient.  The VAE is frozen in the
-    fine-tuning recipe (training/train.py:323-326), so only d/dx is produced."""
+    """VAEAttention (single head, d = channels) + its data gradient, on the path inference takes for the same shape
+    (vae.use_fused_attention): the unfused GEMM + row-softmax path, which saves P [B, L, Lp], or the d=512 flash
+    kernel, which saves Q, K, V, O and the log-sum-exp and recomputes P in the fused backward (O(L) memory).  The VAE
+    is frozen in the fine-tuning recipe (training/train.py:323-326), so only d/dx is produced."""
 
     @staticmethod
     def forward(ctx, m, box, x):
-        out, (hn, qk, p_buf, o) = m.forward_unfused(x)
+        from .vae import use_fused_attention
+        B, H, W, C = x.shape
+        ctx.fused = use_fused_attention(B, H * W, C, m.memory_efficient)
+        out, saved = m.forward_fused(x, want_lse=True) if ctx.fused else m.forward_unfused(x)
         mr = ops.group_norm_mean_rstd(x, m.eps, m.groups)
-        ctx.m, ctx.saved = m, (x, mr, hn, qk, p_buf, o)
+        ctx.m, ctx.saved = m, (x, mr, *saved)
         return _stash(out, box)
 
     @staticmethod
     def backward(ctx, dout):
         m = ctx.m
-        x, mr, hn, qk, p_buf, o = ctx.saved
-        pk = m._packed()
         if any(p.requires_grad for p in m.parameters()):
             raise NotImplementedError("the VAE attention block is differentiable w.r.t. its input only (frozen VAE)")
+        x, mr = ctx.saved[:2]
+        pk = m._packed()
         B, H, W, C = x.shape
-        L = H * W
+        dout = dout.contiguous()
+        dhn = (_VAEAttentionFn._dhn_fused if ctx.fused else _VAEAttentionFn._dhn_unfused)(pk, dout, *ctx.saved[2:])
+        (dx,), _, _ = ops.group_norm_bwd([x], dhn.view(B, H, W, C), mr, pk["g"], pk["b"], m.groups, False, [dout], F32)
+        return None, None, dx
+
+    @staticmethod
+    def _dhn_fused(pk, dout, hn, qkv, o, lse):
+        """d(GroupNorm output) through the out-projection, the fused d=512 attention backward and the QKV projection."""
+        B, L, C = o.shape
+        do, _, _ = bw.linear_bwd(o.view(B * L, C), pk["wo"], ops.cast_f16(dout).view(B * L, C), need_dw=False)
+        do = do.view(B, L, C)
+        delta = ops.rowdot_d512(do, o)
+        dqkv = torch.empty((B, L, 3 * C), dtype=F16, device=o.device)
+        ops.attention_d512_bwd(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], do, lse, delta,
+                               dqkv[..., :C], dqkv[..., C:2 * C], dqkv[..., 2 * C:], C ** -0.5)
+        dhn, _, _ = bw.linear_bwd(hn, pk["wqkv"], dqkv.view(B * L, 3 * C), need_dw=False)
+        return dhn
+
+    @staticmethod
+    def _dhn_unfused(pk, dout, hn, qk, p_buf, o):
+        B, L, C = o.shape
         Lp = p_buf.shape[2]
         scale = C ** -0.5
-        dev = x.device
-        dout = dout.contiguous()
+        dev = o.device
         do, _, _ = bw.linear_bwd(o.view(B * L, C), pk["wo"], ops.cast_f16(dout).view(B * L, C), need_dw=False)
         do = do.view(B, L, C)
         v = ops.linear(hn.view(B * L, C), pk["wv"], pk["bv"]).view(B, L, C)            # recomputed (forward keeps V^T)
@@ -463,8 +487,7 @@ class _VAEAttentionFn(torch.autograd.Function):
             ops.linear(p_buf[b][:, :L], do[b], out=dv[b], a_t=True, w_t=True)
         dhn, _, _ = bw.linear_bwd(hn.view(B * L, C), pk["wqk"], dqk.view(B * L, 2 * C), need_dw=False)
         dhn, _, _ = bw.linear_bwd(hn.view(B * L, C), pk["wv"], dv.view(B * L, C), need_dw=False, da_add=dhn)
-        (dx,), _, _ = ops.group_norm_bwd([x], dhn.view(B, H, W, C), mr, pk["g"], pk["b"], m.groups, False, [dout], F32)
-        return None, None, dx
+        return dhn
 
 
 def vae_attention(m, x):

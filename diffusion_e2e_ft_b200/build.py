@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200_e2eft.so")
 OBJ = os.path.join(HERE, "build")
-SOURCES = ["gemm_conv.cu", "attention.cu", "attention_bwd.cu", "norm.cu", "elementwise.cu", "conv_small.cu", "loss.cu", "optim.cu", "backward.cu", "postproc.cu",
+SOURCES = ["gemm_conv.cu", "attention.cu", "attention_bwd.cu", "attention_d512_bwd.cu", "norm.cu", "elementwise.cu", "conv_small.cu", "loss.cu", "optim.cu", "backward.cu", "postproc.cu",
            "evaluation.cu", "data.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -23,6 +23,7 @@
 //   D = 160      2 warpgroups,  64-key tiles, 3 stages   (Q 48 KB + K/V 144 KB; O 80 + S 32 + P 16 registers)
 #include "attention.cuh"
 #include "../../include/b200_e2eft.h"
+#include "../../include/b200_e2eft_vae_attention.h"
 
 namespace b200 {
 
@@ -263,6 +264,8 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 // (A separate producer warp would make the CTA 288 threads, which the register file serves as 384: 168 each.)
 // Shared memory: Q 64 KB (resident) + 2 x K 32 KB + 2 x V 32 KB + 2 x 2 partial-S tiles of 8 KB = 224 KB + barriers
 // + 1 KB alignment slack, of the 227 KB an sm_90 CTA may use.
+// With `lse` set, warpgroup 0 also stores each row's log2-domain log-sum-exp m c + log2(l) (attention_kernel<D>'s
+// convention), which attention_d512_bwd.cu recomputes P from; O is computed and stored the same way either way.
 constexpr int kD5 = 512;
 constexpr int kD5WG = 2;                          // warpgroups
 constexpr int kD5Cols = kD5 / kD5WG;             // output columns per warpgroup
@@ -282,11 +285,8 @@ struct AttD512Params {
   float scale_log2;
   __half* out;
   long long o_bs, o_ls;
+  float* lse;                  // optional [B][Lq]
 };
-
-__device__ __forceinline__ void named_barrier_sync(int id, int threads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
 
 __device__ __forceinline__ void d512_load_kv(const CUtensorMap* tm, uint64_t* bar, uint8_t* dst, int key0, int b) {
   mbar_arrive_expect_tx(bar, kD5KvBytes);
@@ -448,6 +448,8 @@ attention_d512_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_cons
   for (int r = 0; r < 2; ++r) {
     const int qrow = q0 + r0 + 8 * r;
     if (qrow >= p.Lq) continue;                      // rows past Lq came from TMA zero fill
+    if (p.lse != nullptr && w == 0 && (lane & 3) == 0)   // both warpgroups hold the same m and l
+      p.lse[(long long)b * p.Lq + qrow] = fmaf(m[r], c, log2f(l[r]));
     const float inv = 1.0f / l[r];
     __half* dst = p.out + (long long)b * p.o_bs + (long long)qrow * p.o_ls + w * kD5Cols + cq;
 #pragma unroll
@@ -528,9 +530,10 @@ extern "C" int b200_attention_d64(const void* q, long long q_bs, long long q_ls,
                         kv_segments, scale, lse, stream);
 }
 
-extern "C" int b200_attention_d512(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs,
-                                   long long k_ls, const void* v, long long v_bs, long long v_ls, void* out,
-                                   long long o_bs, long long o_ls, int B, int Lq, int Lk, float scale, void* stream) {
+extern "C" int b200_attention_d512_lse(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs,
+                                       long long k_ls, const void* v, long long v_bs, long long v_ls, void* out,
+                                       long long o_bs, long long o_ls, int B, int Lq, int Lk, float scale, float* lse,
+                                       void* stream) {
   B200_CHECK_ARG(q && k && v && out, "b200_attention_d512: null pointer");
   B200_CHECK_ARG(B > 0 && B <= 65535 && Lq > 0 && Lk > 0, "b200_attention_d512: bad shape B=%d Lq=%d Lk=%d", B, Lq, Lk);
   B200_CHECK_ARG(q_ls % 8 == 0 && k_ls % 8 == 0 && v_ls % 8 == 0 && o_ls % 8 == 0 && q_bs % 8 == 0 &&
@@ -541,24 +544,12 @@ extern "C" int b200_attention_d512(const void* q, long long q_bs, long long q_ls
                  "b200_attention_d512: row strides must be >= 512 elements, batch strides >= 0");
   B200_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) & 15) == 0,
                  "b200_attention_d512: pointers must be 16-byte aligned");
+  B200_CHECK_ARG(((uintptr_t)lse & 3) == 0, "b200_attention_d512: lse must be 4-byte aligned");
   CUtensorMap tq, tk, tv;
-  const uint32_t box[3] = {64, kD5Bq, 1};
-  const uint32_t kv_box[3] = {64, kD5Bk, 1};
-  {
-    uint64_t dims[3] = {(uint64_t)kD5, (uint64_t)Lq, (uint64_t)B};
-    uint64_t str[2] = {(uint64_t)q_ls * 2, (uint64_t)q_bs * 2};
-    int r = encode_tmap(&tq, q, 3, dims, str, box, nullptr);
-    if (r) return r;
-  }
-  {
-    uint64_t dims[3] = {(uint64_t)kD5, (uint64_t)Lk, (uint64_t)B};
-    uint64_t str[2] = {(uint64_t)k_ls * 2, (uint64_t)k_bs * 2};
-    int r = encode_tmap(&tk, k, 3, dims, str, kv_box, nullptr);
-    if (r) return r;
-    uint64_t strv[2] = {(uint64_t)v_ls * 2, (uint64_t)v_bs * 2};
-    r = encode_tmap(&tv, v, 3, dims, strv, kv_box, nullptr);
-    if (r) return r;
-  }
+  int r = encode_d512_tmap(&tq, q, Lq, B, q_ls, q_bs, kD5Bq);
+  if (!r) r = encode_d512_tmap(&tk, k, Lk, B, k_ls, k_bs, kD5Bk);
+  if (!r) r = encode_d512_tmap(&tv, v, Lk, B, v_ls, v_bs, kD5Bk);
+  if (r) return r;
   static bool configured_dev[kMaxDevices] = {false};
   const int dev_ = current_device();
   bool& configured = configured_dev[dev_ < 0 ? 0 : dev_];
@@ -574,8 +565,16 @@ extern "C" int b200_attention_d512(const void* q, long long q_bs, long long q_ls
   p.Lq = Lq; p.Lk = Lk;
   p.scale_log2 = scale * 1.4426950408889634f;
   p.out = (__half*)out; p.o_bs = o_bs; p.o_ls = o_ls;
+  p.lse = lse;
   dim3 grid((Lq + kD5Bq - 1) / kD5Bq, B);
   attention_d512_kernel<<<grid, kD5Threads, kD5Smem, (cudaStream_t)stream>>>(tq, tk, tv, p);
   B200_CHECK_LAUNCH("attention_d512_kernel");
   return 0;
+}
+
+extern "C" int b200_attention_d512(const void* q, long long q_bs, long long q_ls, const void* k, long long k_bs,
+                                   long long k_ls, const void* v, long long v_bs, long long v_ls, void* out,
+                                   long long o_bs, long long o_ls, int B, int Lq, int Lk, float scale, void* stream) {
+  return b200_attention_d512_lse(q, q_bs, q_ls, k, k_bs, k_ls, v, v_bs, v_ls, out, o_bs, o_ls, B, Lq, Lk, scale,
+                                 nullptr, stream);
 }

@@ -74,21 +74,6 @@ struct AttBwdParams {
   long long dq_bs, dq_ls, dk_bs, dk_ls, dv_bs, dv_ls;
 };
 
-// one thread's 64 x 16 A fragment (k-chunk kk) of P and of dS from the accumulator-layout S and dP tiles: element e of
-// column group i sits in row r0 + 8 (e / 2), column 8 i + 2 (lane % 4) + e % 2; lse / nd are per element (the dQ
-// kernel passes its two rows' values, the dK/dV kernel its two columns')
-__device__ __forceinline__ void p_ds_pair(float s0, float s1, float dp0, float dp1, float l0, float l1, float n0,
-                                          float n1, float c, float sc, bool keep0, bool keep1, uint32_t& pa,
-                                          uint32_t& dsa) {
-  const float p0 = keep0 ? ex2_approx(fmaf(s0, c, -l0)) : 0.f;
-  const float p1 = keep1 ? ex2_approx(fmaf(s1, c, -l1)) : 0.f;
-  const __half2 ph = __floats2half2_rn(p0, p1);              // low = p0
-  const float2 pf = __half22float2(ph);
-  const __half2 dh = __floats2half2_rn(fmaf(dp0, sc, n0) * pf.x, fmaf(dp1, sc, n1) * pf.y);
-  pa = *reinterpret_cast<const uint32_t*>(&ph);
-  dsa = *reinterpret_cast<const uint32_t*>(&dh);
-}
-
 // ===================================================================================================== dQ
 template <int D>
 __global__ void __launch_bounds__(kBwdThreads, DqCfg<D>::kMinBlocks)

@@ -126,6 +126,15 @@ _SIGS_ATTENTION_BWD = {
                                    _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_int, c_int, c_int, c_float,
                                    _P]),
 }
+# the VAE mid-block's d=512 attention for training (forward with log-sum-exp, delta, fused backward), declared in
+# include/b200_e2eft_vae_attention.h
+_SIGS_VAE_ATTENTION = {
+    "b200_attention_d512_lse": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int,
+                                        c_float, _P, _P]),
+    "b200_rowdot_d512": (c_int, [_P, _LL, _LL, _P, _LL, _LL, c_int, c_int, _P, _P]),
+    "b200_attention_d512_bwd": (c_int, [_P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _LL, _LL, _P, _P, _P, _LL, _LL,
+                                        _P, _LL, _LL, _P, _LL, _LL, c_int, c_int, c_int, c_float, _P]),
+}
 
 
 def load(build_if_missing=True):
@@ -145,7 +154,7 @@ def load(build_if_missing=True):
     if lib.b200_abi_version() != ABI_VERSION:
         raise RuntimeError(f"{LIB_PATH} exports ABI {lib.b200_abi_version()}, this package binds ABI {ABI_VERSION}: "
                            "rebuild with `python -m diffusion_e2e_ft_b200.build --force`")
-    for name, (res, args) in {**_SIGS, **_SIGS_ATTENTION_BWD}.items():
+    for name, (res, args) in {**_SIGS, **_SIGS_ATTENTION_BWD, **_SIGS_VAE_ATTENTION}.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
         fn.restype = res
         fn.argtypes = args

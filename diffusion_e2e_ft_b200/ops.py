@@ -391,9 +391,11 @@ def attention_bwd(q, k, v, do, lse, delta, dq, dk, dv, heads, scale, kv_segments
 
 
 @_timed("attention")
-def attention_d512(q, k, v, scale, out=None):
+def attention_d512(q, k, v, scale, out=None, want_lse=False):
     """One head of width 512 (VAE mid-block): q [B,Lq,512], k/v [B,Lk,512] fp16 views (last dim contiguous, e.g.
-    slices of one fused [B, L, 1536] projection) -> fp16 [B,Lq,512].  Flash kernel: no L x L buffer."""
+    slices of one fused [B, L, 1536] projection) -> fp16 [B,Lq,512].  Flash kernel: no L x L buffer.
+    `want_lse`: also return the log2-domain log-sum-exp of the scaled scores, fp32 [B, Lq] (P_ij = exp2(scale *
+    log2(e) * S_ij - lse_i)) for `attention_d512_bwd`; the output has the same bits either way."""
     _need_cuda(q, k, v)
     assert q.dtype == F16 and k.dtype == F16 and v.dtype == F16
     assert q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1
@@ -408,11 +410,51 @@ def attention_d512(q, k, v, scale, out=None):
     kb = k.stride(0) if B > 1 else k.stride(1) * Lk
     vb = v.stride(0) if B > 1 else v.stride(1) * Lk
     ob = out.stride(0) if B > 1 else out.stride(1) * Lq
-    rc = _lib.load().b200_attention_d512(_p(q), qb, q.stride(1), _p(k), kb, k.stride(1), _p(v), vb, v.stride(1),
-                                         _p(out), ob, out.stride(1), B, Lq, Lk, float(scale), _stream())
-    _lib.check(rc, "b200_attention_d512")
+    args = (_p(q), qb, q.stride(1), _p(k), kb, k.stride(1), _p(v), vb, v.stride(1), _p(out), ob, out.stride(1),
+            B, Lq, Lk, float(scale))
+    if want_lse:
+        lse = torch.empty((B, Lq), dtype=F32, device=q.device)
+        _lib.check(_lib.load().b200_attention_d512_lse(*args, _p(lse), _stream()), "b200_attention_d512_lse")
+    else:
+        _lib.check(_lib.load().b200_attention_d512(*args, _stream()), "b200_attention_d512")
     STATS.add("attn", 4 * B * Lq * Lk * 512)
+    return (out, lse) if want_lse else out
+
+
+@_timed("bwd_misc")
+def rowdot_d512(a, c):
+    """delta[b, l] = sum_d a[b, l, d] * c[b, l, d] over 512 columns; a, c fp16 [B, L, 512] views (last dim
+    contiguous) -> fp32 [B, L]: the delta = rowsum(dO * O) of `attention_d512_bwd`."""
+    _need_cuda(a, c)
+    assert a.dtype == F16 and c.dtype == F16 and a.stride(-1) == 1 and c.stride(-1) == 1
+    assert a.shape[-1] == 512 and c.shape == a.shape
+    B, L = a.shape[0], a.shape[1]
+    out = torch.empty((B, L), dtype=F32, device=a.device)
+    _ck(_lib.load().b200_rowdot_d512(_p(a), _bstride(a, L), a.stride(1), _p(c), _bstride(c, L), c.stride(1), B, L,
+                                     _p(out), _stream()), "b200_rowdot_d512")
     return out
+
+
+@_timed("attention_bwd")
+def attention_d512_bwd(q, k, v, do, lse, delta, dq, dk, dv, scale):
+    """Fused flash attention backward of `attention_d512` (b200_attention_d512_bwd): q / do / dq [B,Lq,512],
+    k / v / dk / dv [B,Lk,512] fp16 views (last dim contiguous, e.g. column blocks of fused QKV / d(QKV) buffers),
+    lse fp32 [B, Lq] from `attention_d512(..., want_lse=True)`, delta fp32 [B, Lq] from `rowdot_d512(do, out)`.
+    Writes dq, dk, dv; P and dS stay on chip."""
+    _need_cuda(q, k, v, do, dq, dk, dv)
+    B, Lq, Lk = q.shape[0], q.shape[1], k.shape[1]
+    for t, L in ((q, Lq), (k, Lk), (v, Lk), (do, Lq), (dq, Lq), (dk, Lk), (dv, Lk)):
+        assert t.dtype == F16 and t.stride(-1) == 1 and tuple(t.shape) == (B, L, 512), (t.dtype, t.shape, t.stride())
+    assert lse.dtype == F32 and delta.dtype == F32 and lse.is_contiguous() and delta.is_contiguous()
+    assert tuple(lse.shape) == (B, Lq) and tuple(delta.shape) == (B, Lq)
+    rc = _lib.load().b200_attention_d512_bwd(
+        _p(q), _bstride(q, Lq), q.stride(1), _p(k), _bstride(k, Lk), k.stride(1), _p(v), _bstride(v, Lk), v.stride(1),
+        _p(do), _bstride(do, Lq), do.stride(1), _p(lse), _p(delta), _p(dq), _bstride(dq, Lq), dq.stride(1),
+        _p(dk), _bstride(dk, Lk), dk.stride(1), _p(dv), _bstride(dv, Lk), dv.stride(1), B, Lq, Lk, float(scale),
+        _stream())
+    _lib.check(rc, "b200_attention_d512_bwd")
+    STATS.add("attn", 10 * B * Lq * Lk * 512)       # the 5 products of the backward
+    return dq, dk, dv
 
 
 def rowdot_heads(a, c, heads):

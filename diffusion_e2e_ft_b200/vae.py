@@ -47,7 +47,9 @@ class VAEAttention(nn.Module):
       unfused (default): S = QK^T (fp32), row softmax, O = P V^T^T on the wgmma GEMM; V^T comes directly out of a
         swapped-operand GEMM (bias along rows), so no transpose kernel is needed.  Needs 6 B per score (L^2 memory).
       fused (`memory_efficient`, or L too large for the unfused path): one [B*L, 3C] QKV GEMM, the d=512 flash kernel
-        reading Q, K, V in place from it, then the same out-projection.  O(L) memory."""
+        reading Q, K, V in place from it, then the same out-projection.  O(L) memory, in training too: the backward
+        (autograd_blocks._VAEAttentionFn) recomputes P from the saved log-sum-exp in the fused d=512 backward kernels.
+    Training takes the path inference takes (same rule, same forward), so both give the same bits."""
 
     def __init__(self, ch, groups, eps=1e-6):
         super().__init__()
@@ -73,19 +75,25 @@ class VAEAttention(nn.Module):
     def run(self, x, sdt=F32):
         B, H, W, C = x.shape
         if use_fused_attention(B, H * W, C, self.memory_efficient):
-            return self.forward_fused(x, sdt)
+            return self.forward_fused(x, sdt)[0]
         return self.forward_unfused(x, sdt)[0]
 
-    def forward_fused(self, x, sdt=F32):
+    def forward_fused(self, x, sdt=F32, want_lse=False):
+        """The fused path, also returning the intermediates its backward reads: (out, (hn, qkv, o, lse)); lse (the
+        kernel's log2-domain log-sum-exp, [B, L] fp32) only with `want_lse`, else None.  Out is the same either way."""
         pk = self._packed()
         B, H, W, C = x.shape
         L = H * W
         hn = ops.group_norm(x, pk["g"], pk["b"], self.eps, self.groups, False).view(B * L, C)
         qkv = ops.linear(hn, pk["wqkv"], pk["bqkv"]).view(B, L, 3 * C)
-        o = ops.attention_d512(qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:], C ** -0.5)   # [B, L, C]
+        q, k, v = qkv[..., :C], qkv[..., C:2 * C], qkv[..., 2 * C:]
+        if want_lse:
+            o, lse = ops.attention_d512(q, k, v, C ** -0.5, want_lse=True)                  # [B, L, C], [B, L]
+        else:
+            o, lse = ops.attention_d512(q, k, v, C ** -0.5), None
         out = ops.linear(o.view(B * L, C), pk["wo"], pk["bo"], residual=x.view(B * L, C), out_dtype=sdt,
                          stats_rows_per_img=L)
-        return _view_cs(out, B, H, W, C)
+        return _view_cs(out, B, H, W, C), (hn, qkv, o, lse)
 
     def forward_unfused(self, x, sdt=F32):
         """The unfused path, also returning the intermediates its backward reads: (out, (hn, qk, p_buf, o))."""
