@@ -429,13 +429,20 @@ class _VAEAttentionFn(torch.autograd.Function):
     is frozen in the fine-tuning recipe (training/train.py:323-326), so only d/dx is produced."""
 
     @staticmethod
+    def run(m, fused, x):
+        out, saved = m.forward_fused(x, want_lse=True) if fused else m.forward_unfused(x)
+        mr = ops.group_norm_mean_rstd(x, m.eps, m.groups)
+        return out, (x, mr, *saved)
+
+    @staticmethod
     def forward(ctx, m, box, x):
         from .vae import use_fused_attention
         B, H, W, C = x.shape
         ctx.fused = use_fused_attention(B, H * W, C, m.memory_efficient)
-        out, saved = m.forward_fused(x, want_lse=True) if ctx.fused else m.forward_unfused(x)
-        mr = ops.group_norm_mean_rstd(x, m.eps, m.groups)
-        ctx.m, ctx.saved = m, (x, mr, *saved)
+        out, saved = _VAEAttentionFn.run(m, ctx.fused, x)
+        ctx.m = m
+        # gradient checkpointing (B200AutoencoderKL.enable_gradient_checkpointing): keep the input only, as _ResnetFn
+        ctx.saved, ctx.inputs = (None, (ctx.fused, x)) if box.get("ckpt") else (saved, None)
         return _stash(out, box)
 
     @staticmethod
@@ -443,11 +450,12 @@ class _VAEAttentionFn(torch.autograd.Function):
         m = ctx.m
         if any(p.requires_grad for p in m.parameters()):
             raise NotImplementedError("the VAE attention block is differentiable w.r.t. its input only (frozen VAE)")
-        x, mr = ctx.saved[:2]
+        saved = ctx.saved if ctx.saved is not None else _VAEAttentionFn.run(m, *ctx.inputs)[1]
+        x, mr = saved[:2]
         pk = m._packed()
         B, H, W, C = x.shape
         dout = dout.contiguous()
-        dhn = (_VAEAttentionFn._dhn_fused if ctx.fused else _VAEAttentionFn._dhn_unfused)(pk, dout, *ctx.saved[2:])
+        dhn = (_VAEAttentionFn._dhn_fused if ctx.fused else _VAEAttentionFn._dhn_unfused)(pk, dout, *saved[2:])
         (dx,), _, _ = ops.group_norm_bwd([x], dhn.view(B, H, W, C), mr, pk["g"], pk["b"], m.groups, False, [dout], F32)
         return None, None, dx
 
@@ -490,8 +498,8 @@ class _VAEAttentionFn(torch.autograd.Function):
         return dhn
 
 
-def vae_attention(m, x):
-    box = {}
+def vae_attention(m, x, ckpt=False):
+    box = {"ckpt": ckpt}
     return _attach(_VAEAttentionFn.apply(m, box, x), box)
 
 

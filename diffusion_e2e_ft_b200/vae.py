@@ -202,6 +202,7 @@ class Decoder(nn.Module):
         self.conv_out = nn.Conv2d(boc[0], cfg["out_channels"], 3, padding=1)
         self._in = ConvInSmall(self.conv_in)
         self._out = ConvOutSmall(self.conv_norm_out, self.conv_out)
+        self.gradient_checkpointing = False            # B200AutoencoderKL.enable_gradient_checkpointing
 
     def forward(self, z):
         """With grad enabled and `z.requires_grad` every block runs as its autograd Function (autograd_blocks.py);
@@ -214,8 +215,12 @@ class Decoder(nn.Module):
             if sdt != F32:
                 raise NotImplementedError("training runs with the fp32 residual stream (stream_dtype=torch.float32)")
             h = ab.conv_in(self._in, zin)
-            resnet = lambda r, h, f16_copy=False: ab.resnet(r, h, f16_copy=f16_copy)      # noqa: E731
-            attention, upsample = ab.vae_attention, ab.upsample
+            # gradient checkpointing: the resnets and the attention block keep only their inputs.  An upsampler's
+            # backward reads nothing but the fp16 copy of its input that its input carries anyway, so it keeps that.
+            ck = bool(self.gradient_checkpointing)
+            resnet = lambda r, h, f16_copy=False: ab.resnet(r, h, f16_copy=f16_copy, ckpt=ck)  # noqa: E731
+            attention = lambda m, h: ab.vae_attention(m, h, ckpt=ck)                          # noqa: E731
+            upsample = ab.upsample
         else:
             h = self._in.run(zin, sdt)
             resnet = lambda r, h, f16_copy=False: r.run(h, None, None, sdt, f16_copy)     # noqa: E731
@@ -305,6 +310,26 @@ class B200AutoencoderKL(PretrainedMixin, nn.Module):
     @property
     def memory_efficient_attention(self):
         return any(m.memory_efficient for m in self.modules() if isinstance(m, VAEAttention))
+
+    # ---- diffusers' gradient checkpointing switch (ModelMixin.enable_gradient_checkpointing)
+    def enable_gradient_checkpointing(self):
+        """Checkpoint the decoder's blocks: a training forward then keeps only the input of every ResnetBlock2D and of
+        the mid-block attention, and each block re-runs its training forward at the start of its backward, so the
+        decoder's backward needs the block inputs plus one block's intermediates.  The recompute reproduces the saved
+        intermediates bit for bit in practice.  The same kernels run on the same inputs; only the fp64-atomic GroupNorm
+        statistics could round differently.  So the gradients are the plain backward's, bit for bit where that backward
+        reproduces itself; its fp32-atomic sums vary in the last bits run to run.  Per block,
+        not per diffusers segment (mid-block, each up block): at 768 x 768, bs 2 it peaks lower (DESIGN.md §7).  As in
+        current diffusers it applies whenever grad is enabled, also to a frozen VAE in eval mode (the E2E recipes).
+        The encoder has no backward (it runs under no_grad in training), so it has nothing to checkpoint."""
+        self.decoder.gradient_checkpointing = True
+
+    def disable_gradient_checkpointing(self):
+        self.decoder.gradient_checkpointing = False
+
+    @property
+    def is_gradient_checkpointing(self):
+        return any(getattr(m, "gradient_checkpointing", False) for m in self.modules())
 
     # ---- fused conveniences used by the engine's own pipelines (same math as the call sites above)
     def encode_scaled_mean(self, rgb):
