@@ -6,12 +6,19 @@
 //
 //   gather_planar       NHWC -> [C][pixels] transpose with an optional tap shift / stride / nearest-2x source map:
 //                       produces the K-major operands of the weight-gradient GEMMs (K = pixels)
-//   col_sum             bias gradients
+//   col_sum             bias gradients (and the split-K sums of the weight gradients)
 //   gn_mean_rstd        group statistics from the forward's fp64 group sums or per-channel sums
 //   gn_bwd_sums/apply   GroupNorm(+SiLU) backward, two streaming passes
-//   layer_norm_bwd      one warp per row, d_gamma/d_beta through shared-memory then global atomics
+//   layer_norm_bwd      one warp per row, d_gamma/d_beta through per-warp shared-memory rows
 //   softmax_bwd_rows    dS = scale * P o (dP - rowsum(dP o P))
 //   act_bwd / geglu_bwd SiLU / exact-GELU / GEGLU derivatives
+//
+// Reductions across pixels or rows (col_sum, gn_bwd_sums, layer_norm_bwd's d_gamma / d_beta, the loss moments) give
+// one output slot to one thread-block cluster (cluster_reduce.cuh): each CTA reduces a fixed share in a fixed order
+// (thread-sequential, then a fixed xor butterfly or a fixed row order in shared memory, then warps in index order) and
+// rank 0 adds the CTAs' partials in rank order with one plain read-modify-write.  No floating-point atomics; grids and
+// cluster sizes depend only on the problem size, never on the SM count, so a backward pass repeats bit for bit.
+#include "cluster_reduce.cuh"
 #include "common.cuh"
 #include "../../include/b200_e2eft.h"
 
@@ -132,25 +139,39 @@ __global__ void rowdot_heads_kernel(const __half* __restrict__ a, long long a_bs
 }
 
 // ------------------------------------------------------------------------------------------------ col_sum
-// out[c] += sum over rows of x[row][c];  grid (ceil(C/32), row chunks), block (32, 8).
+// out[c] += sum over rows of x[row][c];  grid (ceil(C/32), R), block (32, Y), cluster (1, R): one cluster per 32-column
+// slice.  CTA y of the cluster sums a fixed contiguous share of the rows: thread (c, j) every Y-th row from j, the Y
+// row-threads in order, then rank 0 adds the R CTAs in rank order.  Y = 8, or 32 when the rows span a cluster.
 template <typename T>
-__global__ void col_sum_kernel(const T* __restrict__ x, long long rows, int C, long long ld,
-                               long long rows_per_cta, float* __restrict__ out) {
-  __shared__ float red[8][33];
-  const int c = blockIdx.x * 32 + threadIdx.x;
-  const long long r0 = (long long)blockIdx.y * rows_per_cta;
-  const long long r1 = r0 + rows_per_cta < rows ? r0 + rows_per_cta : rows;
+__global__ void col_sum_kernel(const T* __restrict__ x, long long rows, int C, long long ld, float* __restrict__ out) {
+  __shared__ float red[32][33];
+  const int Y = blockDim.y;
+  const int c0 = blockIdx.x * 32;
+  const int c = c0 + threadIdx.x;
+  long long r0, r1;
+  cluster_share(rows, gridDim.y, blockIdx.y, r0, r1);
+  // one CTA per slot (few rows, e.g. the split-K partials of a weight gradient): the CTA is short, so the old value
+  // of its output is fetched before the loads instead of after the sum
+  const bool alone = gridDim.y == 1;
+  const float old = alone && threadIdx.y == 0 && c < C ? out[c] : 0.f;
   float acc = 0.f;
-  if (c < C)
-    for (long long r = r0 + threadIdx.y; r < r1; r += 8) acc += to_f(x[r * ld + c]);
+  if (c < C) {
+#pragma unroll 4
+    for (long long r = r0 + threadIdx.y; r < r1; r += Y) acc += to_f(x[r * ld + c]);
+  }
   red[threadIdx.y][threadIdx.x] = acc;
   __syncthreads();
-  if (threadIdx.y == 0 && c < C) {
-    float s = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s += red[i][threadIdx.x];
-    atomicAdd(&out[c], s);
+  if (threadIdx.y == 0) {
+    float s = red[0][threadIdx.x];
+    for (int i = 1; i < Y; ++i) s += red[i][threadIdx.x];
+    if (alone) {
+      if (c < C) out[c] = old + s;
+      return;
+    }
+    red[0][threadIdx.x] = s;
   }
+  if (alone) return;
+  cluster_add_partials(&red[0][0], min(32, C - c0), [&](int k) { return out + c0 + k; });
 }
 
 // ------------------------------------------------------------------------------------------ GroupNorm bwd
@@ -183,25 +204,32 @@ __global__ void gn_mean_rstd_kernel(const double* __restrict__ sums, const doubl
 }
 
 // Pass 1: S[n][c_off + c] += (sum dz, sum dz * xhat) over the pixels, dz = dy * silu'(gamma*xhat + beta).
-// x: [NB][HW][Cx] (one of the concatenated inputs, channels c_off.. of the normalised tensor);
-// dy: fp16 [NB][HW][Ctot].  grid (chunks, NB), block V*rpb with V = Cx/8 (same thread map as the forward).
+// x: [NB][HW][Cx] (one of the concatenated inputs, channels c_off.. of the normalised tensor); dy: fp16 [NB][HW][Ctot].
+// grid (R, ceil(Cx/16), NB), cluster (R): one cluster per (image, 16-channel slice); block kGnSumsThreads, thread t
+// owns the 8-channel vector t % 2 of the slice and every (kGnSumsThreads/2)-th pixel of its CTA's contiguous share.
+// Per-thread sums -> xor butterfly over the lanes of the same vector -> warps in order -> ranks in order.
+constexpr int kGnSumsThreads = 512;
 template <typename T>
-__global__ void gn_bwd_sums_kernel(const T* __restrict__ x, int Cx, int c_off, int Ctot,
-                                   const __half* __restrict__ dy, int HW, int groups, int pix_per_cta,
-                                   const float* __restrict__ mr, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, int silu, float* __restrict__ S) {
-  extern __shared__ float sm[];   // [2][Cx]
+__global__ void __launch_bounds__(kGnSumsThreads) gn_bwd_sums_kernel(const T* __restrict__ x, int Cx, int c_off,
+                                                                    int Ctot, const __half* __restrict__ dy, int HW,
+                                                                    int groups, const float* __restrict__ mr,
+                                                                    const float* __restrict__ gamma,
+                                                                    const float* __restrict__ beta, int silu,
+                                                                    float* __restrict__ S) {
+  constexpr int VS = 2, kWarps = kGnSumsThreads / 32, rpb = kGnSumsThreads / VS;
+  __shared__ float red[kWarps][VS * 16];
+  __shared__ float part[VS * 16];
+  const int n = blockIdx.z;
   const int V = Cx / 8;
-  const int n = blockIdx.y;
-  const int rpb = blockDim.x / V;
-  const int v = threadIdx.x % V;
-  const int r = threadIdx.x / V;
-  for (int i = threadIdx.x; i < 2 * Cx; i += blockDim.x) sm[i] = 0.f;
-  __syncthreads();
+  const int vl = threadIdx.x % VS, r = threadIdx.x / VS;
+  const int vg = blockIdx.y * VS + vl;                        // vector index within x's channels
   const int cpg = Ctot / groups;
-  const int c0 = v * 8;
-  if (r < rpb) {
-    float a[8], b[8], rs[8], ms[8], s1[8], s2[8];
+  float s1[8], s2[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) s1[e] = s2[e] = 0.f;
+  if (vg < V) {
+    const int c0 = vg * 8;
+    float a[8], b[8], rs[8], ms[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       const int c = c_off + c0 + e;
@@ -211,16 +239,16 @@ __global__ void gn_bwd_sums_kernel(const T* __restrict__ x, int Cx, int c_off, i
       ms[e] = -mean * rstd;
       a[e] = rstd * gamma[c];
       b[e] = beta[c] - mean * a[e];
-      s1[e] = s2[e] = 0.f;
     }
     const T* xb = x + (long long)n * HW * Cx + c0;
     const __half* db = dy + (long long)n * HW * Ctot + c_off + c0;
-    const int p0 = blockIdx.x * pix_per_cta;
-    const int p1 = min(HW, p0 + pix_per_cta);
-    for (int p = p0 + r; p < p1; p += rpb) {
+    long long p0, p1;
+    cluster_share(HW, gridDim.x, blockIdx.x, p0, p1);
+#pragma unroll 2
+    for (long long p = p0 + r; p < p1; p += rpb) {
       float f[8], d[8];
-      bw_load8(xb + (long long)p * Cx, f);
-      bw_load8(db + (long long)p * Ctot, d);
+      bw_load8(xb + p * Cx, f);
+      bw_load8(db + p * Ctot, d);
 #pragma unroll
       for (int e = 0; e < 8; ++e) {
         const float dz = silu ? d[e] * silu_grad(f[e] * a[e] + b[e]) : d[e];
@@ -228,17 +256,31 @@ __global__ void gn_bwd_sums_kernel(const T* __restrict__ x, int Cx, int c_off, i
         s2[e] += dz * (f[e] * rs[e] + ms[e]);
       }
     }
+  }
 #pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      atomicAdd(&sm[c0 + e], s1[e]);
-      atomicAdd(&sm[Cx + c0 + e], s2[e]);
+  for (int e = 0; e < 8; ++e)
+#pragma unroll
+    for (int o = 16; o >= VS; o >>= 1) {
+      s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], o);
+      s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], o);
+    }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane < VS) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {                              // channel j = 8 lane + e of the slice at [2 j + {0, 1}]
+      red[warp][(8 * lane + e) * 2 + 0] = s1[e];
+      red[warp][(8 * lane + e) * 2 + 1] = s2[e];
     }
   }
   __syncthreads();
-  for (int c = threadIdx.x; c < Cx; c += blockDim.x) {
-    atomicAdd(&S[((long long)n * Ctot + c_off + c) * 2 + 0], sm[c]);
-    atomicAdd(&S[((long long)n * Ctot + c_off + c) * 2 + 1], sm[Cx + c]);
+  if (threadIdx.x < VS * 16) {
+    float t = red[0][threadIdx.x];
+    for (int w = 1; w < kWarps; ++w) t += red[w][threadIdx.x];
+    part[threadIdx.x] = t;
   }
+  const int cs0 = blockIdx.y * VS * 8;                         // first channel of the slice within x
+  cluster_add_partials(part, 2 * min(VS * 8, Cx - cs0),
+                       [&](int k) { return S + ((long long)n * Ctot + c_off + cs0) * 2 + k; });
 }
 
 // Pass 2: dx = rstd * (dz*gamma - A_g - xhat * B_g) (+ add), A_g = mean_g(gamma * dz), B_g = mean_g(gamma * dz * xhat)
@@ -305,20 +347,25 @@ __global__ void gn_bwd_apply_kernel(const T* __restrict__ x, int Cx, int c_off, 
 }
 
 // ------------------------------------------------------------------------------------------ LayerNorm bwd
-// one warp per row (rows strided over the grid); C <= 2048, C % 8 == 0.
-template <typename T, typename TO>
-__global__ void layer_norm_bwd_kernel(const T* __restrict__ x, long long rows, int C,
+// one warp per row; C <= 2048, C % 8 == 0.  grid (R), cluster (R): ONE cluster owns d_gamma / d_beta.  CTA rank k
+// takes a fixed contiguous share of the rows, its warp w every wpb-th row of that share from w; lane l owns the
+// columns of vectors l + 32 i and adds their d_gamma / d_beta terms to the warp's own shared-memory row in row order.
+// The warps' rows are then summed in warp order and the CTAs' in rank order.
+template <typename T, typename TO, int kMaxV>
+__global__ void __launch_bounds__(kMaxV <= 2 ? 1024 : 512) layer_norm_bwd_kernel(const T* __restrict__ x, long long rows, int C,
                                       const float* __restrict__ gamma, const __half* __restrict__ dy, float eps,
                                       const TO* add, TO* dx,
                                       float* __restrict__ dgamma, float* __restrict__ dbeta) {
-  extern __shared__ float sm[];   // dgamma[C], dbeta[C]
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) sm[i] = 0.f;
-  __syncthreads();
+  extern __shared__ float sm[];   // [wpb][2C] per-warp (dgamma, dbeta) rows, then the CTA's [2C] partial
   const int lane = threadIdx.x & 31;
   const int wpb = blockDim.x >> 5;
-  const int V = C / 8;
-  constexpr int kMaxV = 8;
-  for (long long row = (long long)blockIdx.x * wpb + (threadIdx.x >> 5); row < rows; row += (long long)gridDim.x * wpb) {
+  const int V = C / 8;                                       // <= 32 kMaxV vectors of 8 per row
+  for (int i = threadIdx.x; i < wpb * 2 * C; i += blockDim.x) sm[i] = 0.f;
+  __syncthreads();
+  float* wacc = sm + (threadIdx.x >> 5) * 2 * C;
+  long long r0, r1;
+  cluster_share(rows, gridDim.x, blockIdx.x, r0, r1);
+  for (long long row = r0 + (threadIdx.x >> 5); row < r1; row += wpb) {
     float f[kMaxV][8];
     float s = 0.f;
     const T* xr = x + row * C;
@@ -375,18 +422,21 @@ __global__ void layer_norm_bwd_kernel(const T* __restrict__ x, long long rows, i
         for (int e = 0; e < 8; ++e) {
           const float gx = rstd * (d[e] * g[e] - m1 - f[i][e] * m2);
           o[e] = add ? o[e] + gx : gx;
-          atomicAdd(&sm[v * 8 + e], d[e] * f[i][e]);
-          atomicAdd(&sm[C + v * 8 + e], d[e]);
+          wacc[v * 8 + e] += d[e] * f[i][e];
+          wacc[C + v * 8 + e] += d[e];
         }
         bw_store8(dx + row * C + v * 8, o);
       }
     }
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < C; i += blockDim.x) {
-    atomicAdd(&dgamma[i], sm[i]);
-    atomicAdd(&dbeta[i], sm[C + i]);
+  float* part = sm + wpb * 2 * C;
+  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) {
+    float t = sm[i];
+    for (int w = 1; w < wpb; ++w) t += sm[w * 2 * C + i];
+    part[i] = t;
   }
+  cluster_add_partials(part, 2 * C, [&](int k) { return k < C ? dgamma + k : dbeta + (k - C); });
 }
 
 // ------------------------------------------------------------------------------------------- softmax bwd
@@ -448,27 +498,35 @@ __device__ __forceinline__ void ssi_fit(const double* ws, int b, double& s, doub
   s = 0.0; t = 0.0;
   if (det > 0) { s = (a11 * b0 - a01 * b1) / det; t = (-a01 * b0 + a00 * b1) / det; }
 }
-__global__ void ssi_bwd_moments_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
-                                       const uint8_t* __restrict__ mask, long long HW, double* __restrict__ ws) {
+constexpr int kLossBwdThreads = 512;
+// grid (R, B), cluster (R): one cluster per image b (fixed-order sums, cluster_reduce.cuh)
+__global__ void __launch_bounds__(kLossBwdThreads) ssi_bwd_moments_kernel(const float* __restrict__ pred,
+                                                                          const float* __restrict__ tgt,
+                                                                          const uint8_t* __restrict__ mask,
+                                                                          long long HW, double* __restrict__ ws) {
+  __shared__ double part[5];
   const int b = blockIdx.y;
   const float* p = pred + (long long)b * HW;
   const float* y = tgt + (long long)b * HW;
   const uint8_t* m = mask + (long long)b * HW;
-  double a00 = 0, a01 = 0, a11 = 0, b0 = 0, b1 = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
+  double v[5] = {0, 0, 0, 0, 0};
+  long long lo, hi;
+  cluster_share(HW, gridDim.x, blockIdx.x, lo, hi);
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     if (m[i]) {
       const double pv = p[i], yv = y[i];
-      a00 += pv * pv; a01 += pv; a11 += 1.0; b0 += pv * yv; b1 += yv;
+      v[0] += pv * pv; v[1] += pv; v[2] += 1.0; v[3] += pv * yv; v[4] += yv;
     }
   }
-  a00 = bw_warp_sum_d(a00); a01 = bw_warp_sum_d(a01); a11 = bw_warp_sum_d(a11); b0 = bw_warp_sum_d(b0); b1 = bw_warp_sum_d(b1);
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&ws[b * 5 + 0], a00); atomicAdd(&ws[b * 5 + 1], a01); atomicAdd(&ws[b * 5 + 2], a11);
-    atomicAdd(&ws[b * 5 + 3], b0);  atomicAdd(&ws[b * 5 + 4], b1);
-  }
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 5, [&](int k) { return ws + b * 5 + k; });
 }
-__global__ void ssi_bwd_sign_sums_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
-                                         const uint8_t* __restrict__ mask, long long HW, int B, double* __restrict__ ws) {
+__global__ void __launch_bounds__(kLossBwdThreads) ssi_bwd_sign_sums_kernel(const float* __restrict__ pred,
+                                                                            const float* __restrict__ tgt,
+                                                                            const uint8_t* __restrict__ mask,
+                                                                            long long HW, int B,
+                                                                            double* __restrict__ ws) {
+  __shared__ double part[2];
   const int b = blockIdx.y;
   double s, t, det;
   ssi_fit(ws, b, s, t, det);
@@ -476,15 +534,17 @@ __global__ void ssi_bwd_sign_sums_kernel(const float* __restrict__ pred, const f
   const float* p = pred + (long long)b * HW;
   const float* y = tgt + (long long)b * HW;
   const uint8_t* m = mask + (long long)b * HW;
-  double g0 = 0, g1 = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x)
+  double v[2] = {0, 0};
+  long long lo, hi;
+  cluster_share(HW, gridDim.x, blockIdx.x, lo, hi);
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x)
     if (m[i]) {
       const float r = sf * p[i] + tf - y[i];
       const double sg = (r > 0.f) - (r < 0.f);
-      g0 += sg; g1 += sg * (double)p[i];
+      v[0] += sg; v[1] += sg * (double)p[i];
     }
-  g0 = bw_warp_sum_d(g0); g1 = bw_warp_sum_d(g1);
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&ws[5 * B + 2 * b], g0); atomicAdd(&ws[5 * B + 2 * b + 1], g1); }
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 2, [&](int k) { return ws + 5 * B + 2 * b + k; });
 }
 __global__ void ssi_bwd_grad_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
                                     const uint8_t* __restrict__ mask, long long HW, int B, const double* __restrict__ ws,
@@ -520,12 +580,16 @@ __global__ void ssi_bwd_grad_kernel(const float* __restrict__ pred, const float*
 }
 
 // AngularLoss (loss.py:51-67): mean over the mask of acos(clamp(<p, y>, -1, 1)); ws (zeroed double [1]) = count.
-__global__ void mask_count_kernel(const uint8_t* __restrict__ mask, long long n, double* __restrict__ ws) {
-  double c = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    c += mask[i] ? 1.0 : 0.0;
-  c = bw_warp_sum_d(c);
-  if ((threadIdx.x & 31) == 0) atomicAdd(ws, c);
+// grid (R), cluster (R): one cluster counts the whole mask.
+__global__ void __launch_bounds__(kLossBwdThreads) mask_count_kernel(const uint8_t* __restrict__ mask, long long n,
+                                                                     double* __restrict__ ws) {
+  __shared__ double part[1];
+  double c[1] = {0};
+  long long lo, hi;
+  cluster_share(n, gridDim.x, blockIdx.x, lo, hi);
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) c[0] += mask[i] ? 1.0 : 0.0;
+  block_sum_fixed(c, part);
+  cluster_add_partials(part, 1, [&](int) { return ws; });
 }
 __global__ void angular_bwd_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
                                    const uint8_t* __restrict__ mask, long long HW, const double* __restrict__ ws,
@@ -676,19 +740,13 @@ extern "C" int b200_rowdot_heads(const void* a, long long a_bs, long long a_ls, 
 
 extern "C" int b200_col_sum(const void* x, int in_f32, long long rows, int C, long long ld, float* out, void* stream) {
   B200_CHECK_ARG(x && out && rows > 0 && C > 0 && ld >= C, "b200_col_sum: bad arguments");
-  const int cblocks = (C + 31) / 32;
-  long long chunks = ((long long)sm_count() * 8 + cblocks - 1) / cblocks;
-  if (chunks > (rows + 63) / 64) chunks = (rows + 63) / 64;
-  if (chunks < 1) chunks = 1;
-  if (chunks > 65535) chunks = 65535;
-  const long long rpc = (rows + chunks - 1) / chunks;
-  dim3 grid(cblocks, (unsigned)((rows + rpc - 1) / rpc));
-  dim3 block(32, 8);
+  const int R = cluster_ctas(rows, 512);
+  const dim3 grid((C + 31) / 32, R), block(32, R > 1 ? 32 : 8), cluster(1, R, 1);
   cudaStream_t st = (cudaStream_t)stream;
   if (in_f32)
-    col_sum_kernel<float><<<grid, block, 0, st>>>((const float*)x, rows, C, ld, rpc, out);
+    launch_clustered(col_sum_kernel<float>, grid, block, 0, st, cluster, (const float*)x, rows, C, ld, out);
   else
-    col_sum_kernel<__half><<<grid, block, 0, st>>>((const __half*)x, rows, C, ld, rpc, out);
+    launch_clustered(col_sum_kernel<__half>, grid, block, 0, st, cluster, (const __half*)x, rows, C, ld, out);
   B200_CHECK_LAUNCH("col_sum_kernel");
   return 0;
 }
@@ -722,17 +780,15 @@ extern "C" int b200_group_norm_bwd_sums(const void* x, int in_f32, int Cx, int c
   int r = gn_bwd_check("b200_group_norm_bwd_sums", x, Cx, c_off, Ctot, dy, NB, HW, groups);
   if (r) return r;
   B200_CHECK_ARG(mean_rstd && gamma && beta && S, "b200_group_norm_bwd_sums: null pointer");
-  const int T = bw_gn_block(Cx);
-  const int ppc = bw_gn_ppc(NB, HW, T / (Cx / 8));
-  dim3 grid((HW + ppc - 1) / ppc, NB);
-  const size_t smem = 2 * Cx * sizeof(float);
+  const int R = cluster_ctas(HW, 4LL * kGnSumsThreads);
+  const dim3 grid(R, (Cx + 15) / 16, NB), cluster(R, 1, 1);
   cudaStream_t st = (cudaStream_t)stream;
   if (in_f32)
-    gn_bwd_sums_kernel<float><<<grid, T, smem, st>>>((const float*)x, Cx, c_off, Ctot, (const __half*)dy, HW, groups, ppc,
-                                                     mean_rstd, gamma, beta, silu, S);
+    launch_clustered(gn_bwd_sums_kernel<float>, grid, dim3(kGnSumsThreads), 0, st, cluster, (const float*)x, Cx, c_off,
+                     Ctot, (const __half*)dy, HW, groups, mean_rstd, gamma, beta, silu, S);
   else
-    gn_bwd_sums_kernel<__half><<<grid, T, smem, st>>>((const __half*)x, Cx, c_off, Ctot, (const __half*)dy, HW, groups,
-                                                      ppc, mean_rstd, gamma, beta, silu, S);
+    launch_clustered(gn_bwd_sums_kernel<__half>, grid, dim3(kGnSumsThreads), 0, st, cluster, (const __half*)x, Cx, c_off,
+                     Ctot, (const __half*)dy, HW, groups, mean_rstd, gamma, beta, silu, S);
   B200_CHECK_LAUNCH("gn_bwd_sums_kernel");
   return 0;
 }
@@ -766,21 +822,36 @@ extern "C" int b200_layer_norm_bwd(const void* x, int in_f32, long long rows, in
                                    float* dgamma, float* dbeta, void* stream) {
   B200_CHECK_ARG(x && dy && dx && gamma && dgamma && dbeta && rows > 0, "b200_layer_norm_bwd: bad arguments");
   B200_CHECK_ARG(C % 8 == 0 && C <= 2048, "b200_layer_norm_bwd: C=%d must be a multiple of 8 and <= 2048", C);
-  const int wpb = 8;
-  long long grid = (rows + wpb - 1) / wpb;
-  const long long cap = (long long)sm_count() * 8;
-  if (grid > cap) grid = cap;
-  const size_t smem = 2 * C * sizeof(float);
+  // vectors of 8 per lane (the row is held in registers), then warps per CTA: as many per-warp (d_gamma, d_beta) rows
+  // as fit in 200 KB of shared memory, at most 32 (16 with more than 2 vectors per lane: registers)
+  const int nv_need = (C / 8 + 31) / 32;
+  const int nv = nv_need <= 2 ? nv_need : (nv_need <= 5 ? 5 : 8);
+  int wpb = (int)((200 * 1024 / sizeof(float) - 2 * C) / (2 * C));
+  const int wmax = nv <= 2 ? 32 : 16;
+  wpb = wpb < 1 ? 1 : (wpb > wmax ? wmax : wpb);
+  const int R = cluster_ctas(rows, 4LL * wpb, kMaxSingleSlotCtas);
+  const size_t smem = (size_t)(wpb + 1) * 2 * C * sizeof(float);
   cudaStream_t st = (cudaStream_t)stream;
+#define B200_LN_BWD_NV(T_, TO_, NV_)                                                                                 \
+  do {                                                                                                              \
+    cudaFuncSetAttribute(layer_norm_bwd_kernel<T_, TO_, NV_>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
+                         (int)smem);                                                                                \
+    launch_clustered(layer_norm_bwd_kernel<T_, TO_, NV_>, dim3(R), dim3(wpb * 32), smem, st, dim3(R, 1, 1),         \
+                     (const T_*)x, rows, C, gamma, (const __half*)dy, eps, (const TO_*)add, (TO_*)dx, dgamma, dbeta); \
+  } while (0)
 #define B200_LN_BWD(T_, TO_)                                                                                        \
-  layer_norm_bwd_kernel<T_, TO_><<<(unsigned)grid, wpb * 32, smem, st>>>((const T_*)x, rows, C, gamma,              \
-                                                                         (const __half*)dy, eps, (const TO_*)add,  \
-                                                                         (TO_*)dx, dgamma, dbeta)
+  do {                                                                                                              \
+    if (nv == 1) B200_LN_BWD_NV(T_, TO_, 1);                                                                        \
+    else if (nv == 2) B200_LN_BWD_NV(T_, TO_, 2);                                                                   \
+    else if (nv == 5) B200_LN_BWD_NV(T_, TO_, 5);                                                                   \
+    else B200_LN_BWD_NV(T_, TO_, 8);                                                                                \
+  } while (0)
   if (in_f32 && out_f32) B200_LN_BWD(float, float);
   else if (in_f32) B200_LN_BWD(float, __half);
   else if (out_f32) B200_LN_BWD(__half, float);
   else B200_LN_BWD(__half, __half);
 #undef B200_LN_BWD
+#undef B200_LN_BWD_NV
   B200_CHECK_LAUNCH("layer_norm_bwd_kernel");
   return 0;
 }
@@ -827,9 +898,12 @@ extern "C" int b200_ssi_loss_bwd(const float* pred, const float* target, const u
   B200_CHECK_ARG(pred && target && mask && workspace && grad_out && dpred && B > 0 && HW > 0,
                  "b200_ssi_loss_bwd: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
+  const int R = cluster_ctas(HW, 8LL * kLossBwdThreads);
+  launch_clustered(ssi_bwd_moments_kernel, dim3(R, B), dim3(kLossBwdThreads), 0, st, dim3(R, 1, 1), pred, target, mask,
+                   HW, workspace);
+  launch_clustered(ssi_bwd_sign_sums_kernel, dim3(R, B), dim3(kLossBwdThreads), 0, st, dim3(R, 1, 1), pred, target,
+                   mask, HW, B, workspace);
   dim3 grid = bw_loss_grid(HW, B);
-  ssi_bwd_moments_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, workspace);
-  ssi_bwd_sign_sums_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, B, workspace);
   ssi_bwd_grad_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, B, workspace, grad_out, dpred);
   B200_CHECK_LAUNCH("ssi_loss_bwd kernels");
   return 0;
@@ -841,7 +915,9 @@ extern "C" int b200_angular_loss_bwd(const float* pred, const float* target, con
   B200_CHECK_ARG(pred && target && mask && workspace && grad_out && dpred && B > 0 && HW > 0,
                  "b200_angular_loss_bwd: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  mask_count_kernel<<<bw_grid1d((long long)B * HW, 256), 256, 0, st>>>(mask, (long long)B * HW, workspace);
+  const int R = cluster_ctas((long long)B * HW, 8LL * kLossBwdThreads, kMaxSingleSlotCtas);
+  launch_clustered(mask_count_kernel, dim3(R), dim3(kLossBwdThreads), 0, st, dim3(R, 1, 1), mask, (long long)B * HW,
+                   workspace);
   angular_bwd_kernel<<<bw_loss_grid(HW, B), 256, 0, st>>>(pred, target, mask, HW, workspace, grad_out, dpred);
   B200_CHECK_LAUNCH("angular_loss_bwd kernels");
   return 0;

@@ -1,72 +1,89 @@
 // Task losses of the E2E fine-tuning step (forward): scale-and-shift-invariant L1 (depth) and angular (normals).
 // Reference: training/util/loss.py:13-47 (ScaleAndShiftInvariantLoss, compute_scale_and_shift_masked) and
-// :51-67 (AngularLoss), called at training/train.py:542-556.  HBM-bound masked reductions, double atomics.
+// :51-67 (AngularLoss), called at training/train.py:542-556.  HBM-bound masked reductions in fp64.  Every sum is
+// reduced in a fixed order by one thread-block cluster per output slot (cluster_reduce.cuh): thread-sequential over a
+// fixed share of the pixels, a fixed xor butterfly, the warps in index order, then the cluster's CTAs in rank order,
+// added to the zeroed workspace by one plain read-modify-write.  No floating-point atomics; the grid depends only on
+// the problem size, so two runs (on any H100) give the same bits.
+#include "cluster_reduce.cuh"
 #include "common.cuh"
 #include "../../include/b200_e2eft.h"
 
 namespace b200 {
 
-__device__ __forceinline__ double warp_sum_d(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
+constexpr int kLossThreads = 512;
 
-// ws[b*5 + {0..4}] += (sum m p p, sum m p, sum m, sum m p y, sum m y)
-__global__ void ssi_moments_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
-                                   const uint8_t* __restrict__ mask, long long HW, double* __restrict__ ws) {
+// ws[b*5 + {0..4}] += (sum m p p, sum m p, sum m, sum m p y, sum m y); grid (R, B), one cluster per image b
+__global__ void __launch_bounds__(kLossThreads) ssi_moments_kernel(const float* __restrict__ pred,
+                                                                   const float* __restrict__ tgt,
+                                                                   const uint8_t* __restrict__ mask, long long HW,
+                                                                   double* __restrict__ ws) {
+  __shared__ double part[5];
   const int b = blockIdx.y;
   const float* p = pred + (long long)b * HW;
   const float* y = tgt + (long long)b * HW;
   const uint8_t* m = mask + (long long)b * HW;
-  double a00 = 0, a01 = 0, a11 = 0, b0 = 0, b1 = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x) {
+  double v[5] = {0, 0, 0, 0, 0};
+  long long lo, hi;
+  cluster_share(HW, gridDim.x, blockIdx.x, lo, hi);
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     if (m[i]) {
       const double pv = p[i], yv = y[i];
-      a00 += pv * pv; a01 += pv; a11 += 1.0; b0 += pv * yv; b1 += yv;
+      v[0] += pv * pv; v[1] += pv; v[2] += 1.0; v[3] += pv * yv; v[4] += yv;
     }
   }
-  a00 = warp_sum_d(a00); a01 = warp_sum_d(a01); a11 = warp_sum_d(a11); b0 = warp_sum_d(b0); b1 = warp_sum_d(b1);
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&ws[b * 5 + 0], a00); atomicAdd(&ws[b * 5 + 1], a01); atomicAdd(&ws[b * 5 + 2], a11);
-    atomicAdd(&ws[b * 5 + 3], b0);  atomicAdd(&ws[b * 5 + 4], b1);
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 5, [&](int k) { return ws + b * 5 + k; });
+}
+
+// ws[B*5] += sum m |s p + t - y| ; ws[B*5+1] += sum m      with (s,t) the per-image least-squares fit.
+// grid (R): one cluster over the whole batch, each CTA taking the same share of every image, images in order.
+__global__ void __launch_bounds__(kLossThreads) ssi_l1_kernel(const float* __restrict__ pred,
+                                                              const float* __restrict__ tgt,
+                                                              const uint8_t* __restrict__ mask, long long HW, int B,
+                                                              double* __restrict__ ws) {
+  __shared__ double part[2];
+  double v[2] = {0, 0};
+  long long lo, hi;
+  cluster_share(HW, gridDim.x, blockIdx.x, lo, hi);
+  for (int b = 0; b < B; ++b) {
+    const double a00 = ws[b * 5 + 0], a01 = ws[b * 5 + 1], a11 = ws[b * 5 + 2], b0 = ws[b * 5 + 3], b1 = ws[b * 5 + 4];
+    const double det = a00 * a11 - a01 * a01;
+    float s = 0.f, t = 0.f;                                     // loss.py:41-46: only a positive determinant is solved
+    if (det > 0) { s = (float)((a11 * b0 - a01 * b1) / det); t = (float)((-a01 * b0 + a00 * b1) / det); }
+    const float* p = pred + (long long)b * HW;
+    const float* y = tgt + (long long)b * HW;
+    const uint8_t* m = mask + (long long)b * HW;
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x)
+      if (m[i]) { v[0] += fabsf(s * p[i] + t - y[i]); v[1] += 1.0; }
   }
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 2, [&](int k) { return ws + B * 5 + k; });
 }
 
-// ws[B*5] += sum m |s p + t - y| ; ws[B*5+1] += sum m      with (s,t) the per-image least-squares fit
-__global__ void ssi_l1_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
-                              const uint8_t* __restrict__ mask, long long HW, int B, double* __restrict__ ws) {
-  const int b = blockIdx.y;
-  const double a00 = ws[b * 5 + 0], a01 = ws[b * 5 + 1], a11 = ws[b * 5 + 2], b0 = ws[b * 5 + 3], b1 = ws[b * 5 + 4];
-  const double det = a00 * a11 - a01 * a01;
-  float s = 0.f, t = 0.f;                                     // loss.py:41-46: only a positive determinant is solved
-  if (det > 0) { s = (float)((a11 * b0 - a01 * b1) / det); t = (float)((-a01 * b0 + a00 * b1) / det); }
-  const float* p = pred + (long long)b * HW;
-  const float* y = tgt + (long long)b * HW;
-  const uint8_t* m = mask + (long long)b * HW;
-  double acc = 0, cnt = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x)
-    if (m[i]) { acc += fabsf(s * p[i] + t - y[i]); cnt += 1.0; }
-  acc = warp_sum_d(acc); cnt = warp_sum_d(cnt);
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&ws[B * 5], acc); atomicAdd(&ws[B * 5 + 1], cnt); }
-}
-
-__global__ void angular_kernel(const float* __restrict__ pred, const float* __restrict__ tgt,
-                               const uint8_t* __restrict__ mask, long long HW, double* __restrict__ ws) {
-  const int b = blockIdx.y;
-  const float* p = pred + (long long)b * 3 * HW;
-  const float* y = tgt + (long long)b * 3 * HW;
-  const uint8_t* m = mask + (long long)b * HW;
-  double acc = 0, cnt = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += (long long)gridDim.x * blockDim.x)
-    if (m[i]) {
-      float d = p[i] * y[i] + p[HW + i] * y[HW + i] + p[2 * HW + i] * y[2 * HW + i];
-      d = fminf(fmaxf(d, -1.0f), 1.0f);
-      acc += acosf(d);
-      cnt += 1.0;
-    }
-  acc = warp_sum_d(acc); cnt = warp_sum_d(cnt);
-  if ((threadIdx.x & 31) == 0) { atomicAdd(&ws[0], acc); atomicAdd(&ws[1], cnt); }
+// ws[0] += sum m acos(clamp(<p, y>)), ws[1] += sum m; grid (R): one cluster over the whole batch
+__global__ void __launch_bounds__(kLossThreads) angular_kernel(const float* __restrict__ pred,
+                                                               const float* __restrict__ tgt,
+                                                               const uint8_t* __restrict__ mask, long long HW, int B,
+                                                               double* __restrict__ ws) {
+  __shared__ double part[2];
+  double v[2] = {0, 0};
+  long long lo, hi;
+  cluster_share(HW, gridDim.x, blockIdx.x, lo, hi);
+  for (int b = 0; b < B; ++b) {
+    const float* p = pred + (long long)b * 3 * HW;
+    const float* y = tgt + (long long)b * 3 * HW;
+    const uint8_t* m = mask + (long long)b * HW;
+    for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x)
+      if (m[i]) {
+        float d = p[i] * y[i] + p[HW + i] * y[HW + i] + p[2 * HW + i] * y[2 * HW + i];
+        d = fminf(fmaxf(d, -1.0f), 1.0f);
+        v[0] += acosf(d);
+        v[1] += 1.0;
+      }
+  }
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 2, [&](int k) { return ws + k; });
 }
 
 __global__ void mean_finalize_kernel(const double* __restrict__ ws, float* __restrict__ out) {
@@ -76,35 +93,42 @@ __global__ void mean_finalize_kernel(const double* __restrict__ ws, float* __res
 // Masked latent MSE of the diffusion objective (train_depth_normal.py:607-609,712-714).  One thread per latent pixel
 // (b, p): the pixel is valid iff all 64 pixels of its 8x8 block of val_mask are (~max_pool2d(~val_mask, 8, 8), floor
 // cropping); the mask is stored for the backward and, when valid, the squared differences of the 2 halves x C channels
-// of that pixel are summed in fp64.  ws[0] += sum, ws[1] += count (exact in fp64).
+// of that pixel are summed in fp64.  ws[0] += sum, ws[1] += count (exact in fp64).  grid (R): one cluster over the batch.
 template <typename T>
-__global__ void masked_latent_mse_kernel(const T* __restrict__ pred, const float* __restrict__ tgt,
-                                         const uint8_t* __restrict__ vm, int B, int C, int H, int W, int h, int w,
-                                         uint8_t* __restrict__ lm, double* __restrict__ ws) {
-  const int b = blockIdx.y;
+__global__ void __launch_bounds__(kLossThreads) masked_latent_mse_kernel(const T* __restrict__ pred,
+                                                                         const float* __restrict__ tgt,
+                                                                         const uint8_t* __restrict__ vm, int B, int C,
+                                                                         int H, int W, int h, int w,
+                                                                         uint8_t* __restrict__ lm,
+                                                                         double* __restrict__ ws) {
+  __shared__ double part[2];
   const long long hw = (long long)h * w;
-  double acc = 0, cnt = 0;
-  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (long long)gridDim.x * blockDim.x) {
-    const int y = (int)(p / w), x = (int)(p - (long long)y * w);
-    const uint8_t* blk = vm + ((long long)b * H + 8 * y) * W + 8 * x;
-    bool ok = true;
+  double v[2] = {0, 0};
+  long long lo, hi;
+  cluster_share(hw, gridDim.x, blockIdx.x, lo, hi);
+  for (int b = 0; b < B; ++b)
+    for (long long p = lo + threadIdx.x; p < hi; p += blockDim.x) {
+      const int y = (int)(p / w), x = (int)(p - (long long)y * w);
+      const uint8_t* blk = vm + ((long long)b * H + 8 * y) * W + 8 * x;
+      bool ok = true;
 #pragma unroll
-    for (int r = 0; r < 8; ++r)
+      for (int r = 0; r < 8; ++r)
 #pragma unroll
-      for (int s = 0; s < 8; ++s) ok = ok && blk[(long long)r * W + s] != 0;
-    lm[(long long)b * hw + p] = ok;
-    if (ok) {
-      for (int half = 0; half < 2; ++half)
-        for (int c = 0; c < C; ++c) {
-          const long long idx = (((long long)half * B + b) * C + c) * hw + p;
-          const double d = (double)(float)pred[idx] - (double)tgt[idx];
-          acc += d * d;
-        }
-      cnt += 2.0 * C;
+        for (int s = 0; s < 8; ++s) ok = ok && blk[(long long)r * W + s] != 0;
+      lm[(long long)b * hw + p] = ok;
+      if (ok) {
+#pragma unroll 1
+        for (int half = 0; half < 2; ++half)
+          for (int c = 0; c < C; ++c) {
+            const long long idx = (((long long)half * B + b) * C + c) * hw + p;
+            const double d = (double)(float)pred[idx] - (double)tgt[idx];
+            v[0] += d * d;
+          }
+        v[1] += 2.0 * C;
+      }
     }
-  }
-  acc = warp_sum_d(acc); cnt = warp_sum_d(cnt);
-  if ((threadIdx.x & 31) == 0 && cnt > 0) { atomicAdd(&ws[0], acc); atomicAdd(&ws[1], cnt); }
+  block_sum_fixed(v, part);
+  cluster_add_partials(part, 2, [&](int k) { return ws + k; });
 }
 
 __global__ void masked_mean_finalize_kernel(const double* __restrict__ ws, float* __restrict__ out) {
@@ -129,13 +153,9 @@ __global__ void masked_latent_mse_bwd_kernel(const T* __restrict__ pred, const f
   }
 }
 
-static dim3 loss_grid(long long HW, int B) {
-  long long g = (HW + 256 * 8 - 1) / (256 * 8);
-  long long cap = (long long)sm_count() * 4 / (B > 0 ? B : 1) + 1;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return dim3((unsigned)g, B);
-}
+// CTAs per cluster for a reduction over `elems` elements per slot: at least 8 elements per thread; up to 16 CTAs when
+// the whole batch is one slot
+static int loss_ctas(long long elems, int max_ctas) { return cluster_ctas(elems, 8LL * kLossThreads, max_ctas); }
 
 }  // namespace b200
 
@@ -145,9 +165,11 @@ extern "C" int b200_ssi_loss(const float* pred, const float* target, const unsig
                              long long HW, double* workspace, float* out, void* stream) {
   B200_CHECK_ARG(pred && target && mask && workspace && out && B > 0 && HW > 0, "b200_ssi_loss: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid = loss_grid(HW, B);
-  ssi_moments_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, workspace);
-  ssi_l1_kernel<<<grid, 256, 0, st>>>(pred, target, mask, HW, B, workspace);
+  const int R = loss_ctas(HW, kMaxClusterCtas), R1 = loss_ctas((long long)B * HW, kMaxSingleSlotCtas);
+  launch_clustered(ssi_moments_kernel, dim3(R, B), dim3(kLossThreads), 0, st, dim3(R, 1, 1), pred, target, mask, HW,
+                   workspace);
+  launch_clustered(ssi_l1_kernel, dim3(R1), dim3(kLossThreads), 0, st, dim3(R1, 1, 1), pred, target, mask, HW, B,
+                   workspace);
   mean_finalize_kernel<<<1, 1, 0, st>>>(workspace + B * 5, out);
   B200_CHECK_LAUNCH("ssi_loss kernels");
   return 0;
@@ -162,13 +184,14 @@ extern "C" int b200_masked_latent_mse(const void* pred, int pred_f16, const floa
   B200_CHECK_ARG(h == H / 8 && w == W / 8, "b200_masked_latent_mse: latent %dx%d is not the 8x8-pooled mask %dx%d",
                  h, w, H / 8, W / 8);
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid = loss_grid((long long)h * w, B);
+  const int R = loss_ctas((long long)B * h * w, kMaxSingleSlotCtas);
+  const dim3 grid(R), block(kLossThreads), cluster(R, 1, 1);
   if (pred_f16)
-    masked_latent_mse_kernel<__half><<<grid, 256, 0, st>>>((const __half*)pred, target, val_mask, B, C, H, W, h, w,
-                                                           latent_mask, workspace);
+    launch_clustered(masked_latent_mse_kernel<__half>, grid, block, 0, st, cluster, (const __half*)pred, target, val_mask,
+                     B, C, H, W, h, w, latent_mask, workspace);
   else
-    masked_latent_mse_kernel<float><<<grid, 256, 0, st>>>((const float*)pred, target, val_mask, B, C, H, W, h, w,
-                                                          latent_mask, workspace);
+    launch_clustered(masked_latent_mse_kernel<float>, grid, block, 0, st, cluster, (const float*)pred, target, val_mask,
+                     B, C, H, W, h, w, latent_mask, workspace);
   masked_mean_finalize_kernel<<<1, 1, 0, st>>>(workspace, out);
   B200_CHECK_LAUNCH("masked_latent_mse kernels");
   return 0;
@@ -197,7 +220,9 @@ extern "C" int b200_angular_loss(const float* pred, const float* target, const u
                                  long long HW, double* workspace, float* out, void* stream) {
   B200_CHECK_ARG(pred && target && mask && workspace && out && B > 0 && HW > 0, "b200_angular_loss: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  angular_kernel<<<loss_grid(HW, B), 256, 0, st>>>(pred, target, mask, HW, workspace);
+  const int R = loss_ctas((long long)B * HW, kMaxSingleSlotCtas);
+  launch_clustered(angular_kernel, dim3(R), dim3(kLossThreads), 0, st, dim3(R, 1, 1), pred, target, mask, HW, B,
+                   workspace);
   mean_finalize_kernel<<<1, 1, 0, st>>>(workspace, out);
   B200_CHECK_LAUNCH("angular_loss kernels");
   return 0;

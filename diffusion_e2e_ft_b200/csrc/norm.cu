@@ -2,6 +2,7 @@
 // row softmax.  16-byte vectorised coalesced loads, warp-shuffle reductions, fp32 statistics.
 #include <type_traits>
 
+#include "cluster_reduce.cuh"
 #include "common.cuh"
 #include "../../include/b200_e2eft.h"
 
@@ -43,34 +44,35 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // ------------------------------------------------------------------------------ GroupNorm stats
-// grid (chunks, NB); block T = V * rpb where V = C/8 vectors per pixel (each thread owns one fixed
-// 8-channel vector column and strides over pixels).  Per-channel partial sums -> smem -> per-group
-// -> double atomics into sums[n][g][2].
+// sums[n][g] += (sum x, sum x^2) in fp64.  grid (R, slices, NB), cluster (R): one cluster per (image, slice of gs whole
+// groups, gs * C/groups a multiple of 8 channels).  Thread t owns the 8-channel vector t % VS of the slice and every
+// rpb-th pixel of its CTA's contiguous share.  Per-thread sums (shifted, see below) -> a [rpb][2 CS] table in shared
+// memory -> channels summed over the rows in row order -> groups over their channels in order -> the cluster's CTAs
+// in rank order (cluster_reduce.cuh), added to `sums` by rank 0.  No atomics: the bits depend only on the inputs.
 template <typename T>
 __global__ void gn_stats_kernel(const T* __restrict__ x1, int C1, const T* __restrict__ x2, int C2,
-                                int HW, int groups, int pix_per_cta, double* __restrict__ sums) {
-  extern __shared__ double smd[];   // [2][C]
-  const int C = C1 + C2;
-  const int V = C / 8;
-  const int n = blockIdx.y;
-  const int rpb = blockDim.x / V;
-  const int v = threadIdx.x % V;
-  const int r = threadIdx.x / V;
-  for (int i = threadIdx.x; i < 2 * C; i += blockDim.x) smd[i] = 0.0;
-  __syncthreads();
+                                int HW, int groups, int gs, double* __restrict__ sums) {
+  extern __shared__ double smd[];   // [rpb][2 CS] per-thread sums, [2 CS] per-channel sums, [2 gs] group partials
+  const int C = C1 + C2, cpg = C / groups, CS = gs * cpg, VS = CS / 8;
+  const int n = blockIdx.z;
+  const int g0 = blockIdx.y * gs, ng = min(gs, groups - g0);
+  const int rpb = blockDim.x / VS;
+  const int v = threadIdx.x % VS;
+  const int r = threadIdx.x / VS;
   // per-thread sums of (x - shift), (x - shift)^2 with shift = the thread's first element of each channel:
   // no cancellation for |mean| >> std; converted to plain sums in fp64 before merging
   float s[8], q[8], sh[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) s[e] = q[e] = sh[e] = 0.f;
   int cnt = 0;
-  const int p0 = blockIdx.x * pix_per_cta;
-  const int p1 = min(HW, p0 + pix_per_cta);
-  const int c0 = v * 8;
+  long long lp0, lp1;
+  cluster_share(HW, gridDim.x, blockIdx.x, lp0, lp1);
+  const int p0 = (int)lp0, p1 = (int)lp1;
+  const int c0 = g0 * cpg + v * 8;
   const bool second = c0 >= C1;
   const T* base = second ? x2 + (long long)n * HW * C2 + (c0 - C1) : x1 + (long long)n * HW * C1 + c0;
   const int ld = second ? C2 : C1;
-  if (r < rpb) {
+  if (v * 8 < ng * cpg) {
     int p = p0 + r;
     if (p < p1) load8(base + (long long)p * ld, sh);
     for (; p + 3 * rpb < p1; p += 4 * rpb) {
@@ -90,24 +92,30 @@ __global__ void gn_stats_kernel(const T* __restrict__ x1, int C1, const T* __res
       for (int e = 0; e < 8; ++e) { const float d = f[e] - sh[e]; s[e] += d; q[e] = fmaf(d, d, q[e]); }
       cnt += 1;
     }
-    if (cnt) {
-      const double nn = (double)cnt;
+  }
+  const double nn = (double)cnt;
 #pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        const double shd = (double)sh[e], s1 = (double)s[e];
-        atomicAdd(&smd[c0 + e], s1 + nn * shd);
-        atomicAdd(&smd[C + c0 + e], (double)q[e] + 2.0 * shd * s1 + nn * shd * shd);
-      }
-    }
+  for (int e = 0; e < 8; ++e) {
+    const double shd = (double)sh[e], s1 = (double)s[e];
+    smd[(long long)r * 2 * CS + (v * 8 + e) * 2 + 0] = s1 + nn * shd;
+    smd[(long long)r * 2 * CS + (v * 8 + e) * 2 + 1] = (double)q[e] + 2.0 * shd * s1 + nn * shd * shd;
   }
   __syncthreads();
-  const int cg = C / groups;
-  for (int g = threadIdx.x; g < groups; g += blockDim.x) {
-    double a = 0.0, b = 0.0;
-    for (int c = g * cg; c < (g + 1) * cg; ++c) { a += smd[c]; b += smd[C + c]; }
-    atomicAdd(&sums[((long long)n * groups + g) * 2 + 0], a);
-    atomicAdd(&sums[((long long)n * groups + g) * 2 + 1], b);
+  double* ch = smd + (long long)rpb * 2 * CS;
+  for (int k = threadIdx.x; k < 2 * CS; k += blockDim.x) {
+    double t = smd[k];
+    for (int rr = 1; rr < rpb; ++rr) t += smd[(long long)rr * 2 * CS + k];
+    ch[k] = t;
   }
+  __syncthreads();
+  double* part = ch + 2 * CS;
+  for (int k = threadIdx.x; k < 2 * ng; k += blockDim.x) {
+    const int g = k >> 1, f = k & 1;
+    double t = 0.0;
+    for (int c = g * cpg; c < (g + 1) * cpg; ++c) t += ch[c * 2 + f];
+    part[k] = t;
+  }
+  cluster_add_partials(part, 2 * ng, [&](int k) { return sums + ((long long)n * groups + g0) * 2 + k; });
 }
 
 // ------------------------------------------------------------------------------ GroupNorm apply
@@ -497,16 +505,29 @@ extern "C" int b200_group_norm_stats(const void* x1, int C1, const void* x2, int
   int r = gn_common_check("b200_group_norm_stats", x1, C1, x2, C2, NB, HW, groups);
   if (r) return r;
   B200_CHECK_ARG(sums, "b200_group_norm_stats: null sums");
-  const int C = C1 + C2;
-  const int T = gn_block(C);
-  const int ppc = gn_chunks(NB, HW, T / (C / 8));
-  dim3 grid((HW + ppc - 1) / ppc, NB);
-  const size_t smem = 2 * C * sizeof(double);
+  // slices of gs whole groups: the fewest groups whose channels fill 8-channel vectors, doubled up to 16 channels
+  const int cpg = (C1 + C2) / groups;
+  int gs = 1;
+  while ((gs * cpg) % 8 != 0) ++gs;
+  while (2 * gs * cpg <= 16 && 2 * gs <= groups) gs *= 2;
+  const int VS = gs * cpg / 8;
+  const int rpb = VS >= 256 ? 1 : 256 / VS;
+  const int T = VS * rpb;
+  const int R = cluster_ctas(HW, 16LL * rpb);
+  const dim3 grid(R, (groups + gs - 1) / gs, NB), cluster(R, 1, 1);
+  const size_t smem = ((size_t)(rpb + 1) * 2 * gs * cpg + 2 * gs) * sizeof(double);
   cudaStream_t st = (cudaStream_t)stream;
-  if (in_f32)
-    gn_stats_kernel<float><<<grid, T, smem, st>>>((const float*)x1, C1, (const float*)x2, C2, HW, groups, ppc, sums);
-  else
-    gn_stats_kernel<__half><<<grid, T, smem, st>>>((const __half*)x1, C1, (const __half*)x2, C2, HW, groups, ppc, sums);
+  if (in_f32) {
+    if (smem > 48 * 1024)
+      cudaFuncSetAttribute(gn_stats_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    launch_clustered(gn_stats_kernel<float>, grid, dim3(T), smem, st, cluster, (const float*)x1, C1, (const float*)x2,
+                     C2, HW, groups, gs, sums);
+  } else {
+    if (smem > 48 * 1024)
+      cudaFuncSetAttribute(gn_stats_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    launch_clustered(gn_stats_kernel<__half>, grid, dim3(T), smem, st, cluster, (const __half*)x1, C1,
+                     (const __half*)x2, C2, HW, groups, gs, sums);
+  }
   B200_CHECK_LAUNCH("gn_stats_kernel");
   return 0;
 }

@@ -3,24 +3,32 @@
 // `clip_grad_norm_` and a fused clip + AdamW update.  Reference: training/train.py:346-353 (AdamW:
 // lr 3e-5, betas (0.9, 0.999), weight_decay 1e-2, eps 1e-8) and :564-566 (clip to max_grad_norm, step).
 // HBM-bound: 16 B read + 12 B written per parameter.
+#include "cluster_reduce.cuh"
 #include "common.cuh"
 #include "../../include/b200_e2eft.h"
 
 namespace b200 {
 
-__global__ void sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out) {
-  double acc = 0;
+// *out += sum x^2 in fp64.  One cluster of CTAs: CTA `rank` sums a fixed contiguous share of the float4s
+// thread-sequentially (the last CTA also takes the n % 4 tail), block_sum_fixed combines the threads and rank 0 adds the
+// CTAs' partials in rank order (cluster_reduce.cuh): the same bits on every run and every H100.
+__global__ void __launch_bounds__(1024) sumsq_kernel(const float* __restrict__ x, long long n, double* __restrict__ out) {
+  __shared__ double part[1];
+  const int rank = (int)cooperative_groups::this_cluster().block_rank(), R = gridDim.x;
+  double acc[1] = {0.0};
   const long long n4 = n / 4;
+  long long lo, hi;
+  cluster_share(n4, R, rank, lo, hi);
   const float4* x4 = reinterpret_cast<const float4*>(x);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+#pragma unroll 4
+  for (long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
     const float4 v = x4[i];
-    acc += (double)v.x * v.x + (double)v.y * v.y + (double)v.z * v.z + (double)v.w * v.w;
+    acc[0] += (double)v.x * v.x + (double)v.y * v.y + (double)v.z * v.z + (double)v.w * v.w;
   }
-  for (long long i = n4 * 4 + (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    acc += (double)x[i] * x[i];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) atomicAdd(out, acc);
+  if (rank == R - 1)
+    for (long long i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) acc[0] += (double)x[i] * x[i];
+  block_sum_fixed(acc, part);
+  cluster_add_partials(part, 1, [&](int) { return out; });
 }
 
 // torch.optim.AdamW (decoupled weight decay, bias-corrected), gradient pre-scaled by the clip coefficient
@@ -240,9 +248,8 @@ extern "C" int b200_adamw_step_state(float* param, const float* grad, float* exp
 
 extern "C" int b200_sumsq(const float* x, long long n, double* out, void* stream) {
   B200_CHECK_ARG(x && out && n > 0 && ((uintptr_t)x & 15) == 0, "b200_sumsq: bad arguments (x must be 16-byte aligned)");
-  long long g = (n / 4 + 255) / 256;
-  long long cap = (long long)sm_count() * 8;
-  sumsq_kernel<<<(unsigned)(g < 1 ? 1 : (g > cap ? cap : g)), 256, 0, (cudaStream_t)stream>>>(x, n, out);
+  const int R = cluster_ctas(n / 4, 1024LL * 16, kMaxSingleSlotCtas);
+  launch_clustered(sumsq_kernel, dim3(R), dim3(1024), 0, (cudaStream_t)stream, dim3(R, 1, 1), x, n, out);
   B200_CHECK_LAUNCH("sumsq_kernel");
   return 0;
 }

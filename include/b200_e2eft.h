@@ -99,7 +99,7 @@ int b200_im2col3x3_nchw(const void* x, int x_f32, int NB, int C, int H, int W, v
 
 /* GroupNorm statistics over NHWC input that is the channel-concatenation of up to two tensors
  * (skip-connection concat, unet_2d_blocks.py:2328,2456, is never materialised).
- * sums[n][g][2] (double) must be zeroed by the caller. */
+ * sums[n][g][2] (double) must be zeroed by the caller; it receives fixed-order sums (no atomics, same bits every run). */
 int b200_group_norm_stats(const void* x1, int C1, const void* x2, int C2, int in_f32, int NB,
                           int HW, int groups, double* sums, void* stream);
 /* y = [silu]( (x-mean)*rstd*gamma + beta ) as fp16 NHWC; optional raw fp16 copy of the
@@ -225,14 +225,16 @@ int b200_decode_post(const float* x, int NB, long long HW, int mode, float sign,
 
 /* Task losses of the E2E fine-tuning step, forward only (training/util/loss.py:13-67, training/train.py:542-556).
  * pred/target NCHW fp32 ([B][1][HW] depth, [B][3][HW] normals), mask [B][HW] bytes, workspace: zeroed doubles
- * (5*B + 2 for SSI, 2 for angular), out: one float (mean over masked pixels; nan for an empty mask). */
+ * (5*B + 2 for SSI, 2 for angular), out: one float (mean over masked pixels; nan for an empty mask).  Every sum here
+ * and in the loss backward entry points is reduced in a fixed order (no floating-point atomics): the same bits on
+ * every run. */
 int b200_ssi_loss(const float* pred, const float* target, const unsigned char* mask, int B, long long HW,
                   double* workspace, float* out, void* stream);
 int b200_angular_loss(const float* pred, const float* target, const unsigned char* mask, int B, long long HW,
                       double* workspace, float* out, void* stream);
 
 /* Optimizer side of the fine-tuning step on flat fp32 buffers (training/train.py:346-353,564-566):
- * sum of squares (gradient norm; `out` is a zeroed double accumulated with atomics) and a fused
+ * sum of squares (gradient norm; `*out += sum x^2`, a fixed-order fp64 sum: two runs give the same bits) and a fused
  * clip_grad_norm_ + torch.optim.AdamW update (decoupled weight decay, bias correction by `step` >= 1).
  * grad_norm_sq (device, may be NULL) and max_grad_norm give the clip coefficient without a host sync. */
 int b200_sumsq(const float* x, long long n, double* out, void* stream);
@@ -280,6 +282,8 @@ int b200_adamw_step_state_groups(float* param, const float* grad, float* exp_avg
  *   x[n][(stride*o + oy)/up][(stride*p + ox)/up][c] (pixel stride ldx >= C) with q = (n*Ho + o)*Wo + p, zero outside the (up-sampled)
  *   image: the K-major (K = pixels) operand of a weight-gradient GEMM for one kernel tap of a stride-1/-2 or
  *   nearest-2x-upsampled 3x3 conv; with Ho=H, Wo=W, stride=1, up=1, oy=ox=0 a plain [rows][C] -> [C][rows] transpose.
+ * The reductions below (col_sum, group_norm_bwd_sums, layer_norm_bwd's d_gamma/d_beta) sum in a fixed order that
+ * depends only on the shapes (no floating-point atomics), so a backward pass repeats bit for bit.
  * b200_col_sum: out[c] += sum_rows x[row][c] (bias gradients).
  * GroupNorm backward (diffusers GroupNorm(32) + optional SiLU, NHWC): mean_rstd [NB][groups][2] from the
  *   forward's statistics; pass 1 accumulates S [NB][Ctot][2] = (sum dz, sum dz*xhat) per channel (zeroed by
