@@ -247,7 +247,8 @@ int b200_adamw_step_scaled(float* param, const float* grad, float* exp_avg, floa
                            const double* grad_norm_sq, float max_grad_norm, float grad_unscale, void* stream);
 
 /* Same update driven by a device-side state block (fp32[8]: loss scale, growth tracker, applied steps, skipped
- * steps, skipped flag, gradient multiplier, bc1, bc2) so that neither the skip decision nor dynamic loss scaling
+ * steps, skipped flag, gradient multiplier, bc1, bc2 — bc_k = 1 - beta_k^step evaluated in fp64 and rounded to fp32
+ * once, as b200_adamw_step_scaled does on the host) so that neither the skip decision nor dynamic loss scaling
  * needs a host sync: the step is skipped (parameters and moments untouched, as torch.optim.AdamW leaves parameters
  * whose .grad is None) when the gradient norm is non-finite (fp16 overflow of the loss-scaled backward: the scale is
  * halved) or exactly zero (empty validity masks / NaN loss: training/train.py:503,546-551 back-propagates 0).
@@ -324,7 +325,9 @@ int b200_geglu_bwd(const void* h, const void* g, long long ld_hg, const void* dy
 /* Loss / post-op backward of the fine-tuning step (training/train.py:532-556, training/util/loss.py):
  * d(loss)/d(pred) * grad_out[0] (device scalar: the upstream gradient, i.e. the loss scale).  The SSI gradient
  * flows through the per-image least-squares scale/shift, as torch.autograd does in the reference.
- * workspace: zeroed doubles, 7*B (ssi) / 1 (angular).  decode_post_bwd: modes 2 (depth) / 3 (normals). */
+ * workspace: zeroed doubles, 7*B (ssi) / 1 (angular).  decode_post_bwd: modes 2 (depth) / 3 (normals).
+ * b200_angular_loss_bwd returns 0 where the fp32 <pred, target> is -1 or 1 (or beyond): torch's inclusive clamp
+ * passes the gradient there and acos' makes it -inf / NaN, which would only make the optimizer skip the step. */
 int b200_ssi_loss_bwd(const float* pred, const float* target, const unsigned char* mask, int B, long long HW,
                       double* workspace, const float* grad_out, float* dpred, void* stream);
 int b200_angular_loss_bwd(const float* pred, const float* target, const unsigned char* mask, int B, long long HW,
